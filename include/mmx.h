@@ -156,9 +156,11 @@ int mmx_bmm_add(const float* A, int lda, long long strideA, int transA, const fl
 #define MMX_ACT_TANH       4   /* LXMERT pooler, lxmert/lxmert/src/lxmert_lrp.py:868-884 */
 #define MMX_ACT_MUL        5   /* not an activation: the `pre` operand of a GEMM epilogue multiplies the product itself
                                   (C = (A W^T) (.) pre), the `x * (S W)` step of Linear.relprop, DETR/modules/layers.py:421-423 */
+#define MMX_ACT_SIGMOID    6   /* 1/(1+exp(-x)): DETR's box head, `self.bbox_embed(hs).sigmoid()` DETR/models/detr.py:73 */
 
 /* C[M,N] = A[M,K] * W[N,K]^T (+ bias[N]) (+ residual[M,N]);  if act != NONE and C_act != NULL also writes
- * C_act = act(C).  F.linear of CLIP/clip/auxilary.py:77,255 and CLIP/clip/model.py:175-177. */
+ * C_act = act(C); C_act == C stores act(C) only (a forward-only consumer that never needs the pre-activation).
+ * F.linear of CLIP/clip/auxilary.py:77,255 and CLIP/clip/model.py:175-177. */
 int mmx_linear(const float* A, int lda, const float* W, int ldw, const float* bias, const float* residual,
                int ldres, float* C, int ldc, float* C_act, int act, int M, int N, int K, void* stream);
 /* dX[M,K] = (dY[M,N] * W[N,K]) (.) act'(pre[M,K])   given Wt = W^T stored [K,N]:  the dgrad of mmx_linear,
@@ -240,6 +242,36 @@ int mmx_attention_bwd(const float* dO, int lddo, const float* Q, int ldq, const 
                       const float* V, int ldv, const float* A, float* dA, int ldA, float* delta,
                       float* dQ, int lddq, float* dK, int lddk, float* dV, int lddv,
                       int B, int H, int T, int S, int hd, float scale, int flags, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------
+ * DETR backbone from images (SURVEY.md §8a rows a10, a11): the ResNet body, input_proj and the mask / sine position
+ * embedding that DETR.forward runs before the transformer (DETR/models/detr.py:63-69, DETR/models/backbone.py:68-121).
+ * Activations are NHWC matrices [B*H*W, C] (row = (b*H + y)*W + x) with a row stride in elements.
+ * ------------------------------------------------------------------------------------------------------- */
+
+/* out[B*Ho*Wo, Cout] = act(conv2d(x, W) + bias (+ residual)), Ho = (H + 2 pad - kh) / stride + 1 (same for Wo), zero
+ * padding.  Replaces the Conv2d + FrozenBatchNorm2d (+ ReLU, + identity add) steps of torchvision's ResNet
+ * (DETR/models/backbone.py:45-55,91-93) and DETR's input_proj (DETR/models/detr.py:44,69) once the BN affine is folded
+ * into W and bias.  x is addressed through element strides (sN, sY, sX, sC) - an NCHW image and an NHWC activation with
+ * any row stride are both valid inputs.  W: [Cout, kh*kw*C] in (ky, kx, c) order (row stride ldw), packed: its
+ * mmx_pack_weight copy or NULL.  A 1x1 stride-1 conv over rows with unit channel stride is a plain mmx_gemm_nt; every
+ * other conv gathers its [B*Ho*Wo, kh*kw*C] operand once (under backend 3 straight into the fp16 hi / lo planes the
+ * GEMM loads, elsewhere as fp32) into stream-ordered scratch.  act: MMX_ACT_*; the pre-activation is not stored.
+ * residual: [B*Ho*Wo, Cout] (row stride ldres) or NULL. */
+int mmx_conv2d(const float* x, long long sN, long long sY, long long sX, long long sC, int B, int H, int W, int C,
+               const float* Wr, int ldw, const void* packed, const float* bias, const float* residual, int ldres, float* out,
+               int ldo, int Cout, int kh, int kw, int stride, int pad, int act, void* stream);
+/* 3x3 / stride 2 / padding 1 max-pool over NHWC rows (padding acts as -inf, NaN propagates): torchvision ResNet's
+ * maxpool (F.max_pool2d).  in: [B*H*W, C] (ldi), out: [B*Ho*Wo, C] (ldo), Ho = (H - 1) / 2 + 1. */
+int mmx_maxpool2d_nhwc(const float* in, int ldi, float* out, int ldo, int B, int H, int W, int C, void* stream);
+/* The padding mask at feature resolution and PositionEmbeddingSine(npf, temperature, normalize=True) of it, in one kernel.
+ * mask: [B, Hi, Wi] bytes, non-zero = padding (NULL: no padding); it is sampled to [B, h, w] as F.interpolate(mode=
+ * "nearest") does (DETR/models/backbone.py:78) and written to mask_out (bytes, may be NULL).  pos: [B*h*w, 2*npf] (row
+ * stride ldpos, row = (b*h + y)*w + x, the layout the encoder reads), channels [0, npf) from y, [npf, 2 npf) from x,
+ * sin / cos interleaved, in the reference's fp32 operation order (DETR/models/position_encoding.py:28-48).  h*w <= 16384;
+ * one CTA per 32 positions of an image. */
+int mmx_detr_position_sine(const uint8_t* mask, int B, int Hi, int Wi, int h, int w, int npf, float temperature, float* pos,
+                           int ldpos, uint8_t* mask_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * CLIP engine: the north-star path (SURVEY.md §8a rows a1-a4), one call = interpret() for a batch.

@@ -97,5 +97,14 @@ for S_, hd_ in ((197, 64), (300, 32), (850, 16)):                               
                               C.c_float(hd_ ** -0.5), 0, current_stream()))
 gr = g.capture((src.cuda(), pos.cuda()), tq, use_lrp=False)
 gr(src.cuda(), pos.cuda(), tq.cuda()); gr.check()
+# ---- DETR from images (conv.cu): im2col into fp16 planes (backend 3) and into fp32 (backend 1), NCHW stem, strided 1x1,
+# max-pool, mask / position embedding with padding, sigmoid box head
+from oracle import detr_backbone_oracle as dbo
+ieng = mmx_b200.DetrEngine(dbo.init_state_dict(dbo.DETR_IMAGE, 3), nhead=dbo.DETR_IMAGE.nhead, device="cuda:0")
+ims = [torch.randn(3, 70, 90, device="cuda"), torch.randn(3, 64, 100, device="cuda")]
+for backend in (3, 1):
+    l.mmx_set_gemm_backend(backend)
+    ieng(ims)
+mmx_b200.Generator(ieng).generate_ours(ims, torch.tensor([0, 1]), use_lrp=False)
 torch.cuda.synchronize()
 print("sanitize_run: all kernels executed")

@@ -19,6 +19,7 @@ from .synthetic import (clip_init_state_dict, clip_synthetic_inputs, DetrConfig,
                         lxmert_init_state_dict, lxmert_synthetic_inputs)
 from .vit import ViTEngine, generate_relevance  # noqa: F401
 from .detr import DetrEngine, Generator, GeneratorAlbationNoAgg, MaskGenerator  # noqa: F401
+from .backbone import DetrBackbone  # noqa: F401
 from .lxmert import LxmertEngine, GeneratorOurs, GeneratorBaselines, GeneratorOursAblationNoAggregation  # noqa: F401
 from .visualbert import VisualBertEngine, SelfAttentionGenerator  # noqa: F401
 from .perturbation import LxmertPerturbation, VisualBertPerturbation, PERT_STEPS, topk_select  # noqa: F401

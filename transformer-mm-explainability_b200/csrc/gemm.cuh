@@ -10,7 +10,7 @@ struct GemmEpilogue {
   int ldpre = 0;
   const float* residual = nullptr;  // [M,N]: added last
   int ldres = 0;
-  float* C_act = nullptr;           // [M,N] (row stride ldc): also store act(C)
+  float* C_act = nullptr;           // [M,N] (row stride ldc): also store act(C); C_act == C stores act(C) only
   int act = MMX_ACT_NONE;
   const int* m_dev = nullptr;       // optional device-resident row count (<= M): M becomes an upper bound (ragged batches)
 };
@@ -48,6 +48,15 @@ bool gemm_f16x3_shape_ok(const float* A, int lda, const BOperand& B, float* C, i
 // presplit = true: backend 3 (A split into fp16 planes by a separate pass before the kernel)
 int gemm_nt_f16x3(const float* A, int lda, const BOperand& B, float* C, int ldc, int M, int N, int K, const GemmEpilogue& ep,
                   cudaStream_t st, bool presplit = false);
+// The backend-3 kernel on an A that is already split into fp16 hi / lo' planes [M, ldpa] (the conv gather writes them):
+// same kernel and arithmetic as gemm_nt_f16x3(presplit = true) after its split pass.  The planes must be 16-byte aligned
+// (the stream-ordered scratch they live in is); gemm_f16x3_planes_ok checks everything else.
+bool gemm_f16x3_planes_ok(int ldpa, const BOperand& B, float* C, int ldc, int N, int K, const GemmEpilogue& ep);
+int gemm_nt_f16x3_planes(const uint16_t* Ahi, const uint16_t* Alo, int ldpa, const BOperand& B, float* C, int ldc, int M, int N,
+                         int K, const GemmEpilogue& ep, cudaStream_t st);
+// gemm_nt_f16x3_planes inside the mmx_profile_gemm window (gemm_dispatch.cu)
+int gemm_nt_planes(const uint16_t* Ahi, const uint16_t* Alo, int ldpa, const BOperand& B, float* C, int ldc, int M, int N, int K,
+                   const GemmEpilogue& ep, cudaStream_t st);
 
 int gemm_tc_available();
 int gemm_tc_tile_n(int bn);   // forced tensor-core tile width: bn < 0 reads it, 0 = automatic, 128/144/160 force

@@ -83,10 +83,10 @@ int gemm_nt(const float* A, int lda, const float* Bt, int ldb, float* C, int ldc
   return gemm_nt_b(A, lda, B, C, ldc, M, N, K, ep, st);
 }
 
-int gemm_nt_b(const float* A, int lda, const BOperand& Bop, float* C, int ldc, int M, int N, int K, const GemmEpilogue& ep,
-              cudaStream_t st) {
-  if (!g_prof_on.load(std::memory_order_relaxed) || M == 0 || N == 0)
-    return gemm_nt_impl(A, lda, Bop, C, ldc, M, N, K, ep, st);
+// run(): one GEMM launch sequence; timed by CUDA events when a profiling window is open
+template <typename Run>
+static int profiled(int M, int N, int K, const GemmEpilogue& ep, cudaStream_t st, Run run) {
+  if (!g_prof_on.load(std::memory_order_relaxed) || M == 0 || N == 0) return run();
   ProfRec r;
   {
     std::lock_guard<std::mutex> lk(g_prof_mu);
@@ -99,11 +99,21 @@ int gemm_nt_b(const float* A, int lda, const BOperand& Bop, float* C, int ldc, i
   r.m_dev = ep.m_dev;
   r.M = M;
   MMX_CHECK_CUDA(cudaEventRecord(r.s, st));
-  MMX_TRY(gemm_nt_impl(A, lda, Bop, C, ldc, M, N, K, ep, st));
+  MMX_TRY(run());
   MMX_CHECK_CUDA(cudaEventRecord(r.e, st));
   std::lock_guard<std::mutex> lk(g_prof_mu);
   g_prof.push_back(r);
   return 0;
+}
+
+int gemm_nt_b(const float* A, int lda, const BOperand& Bop, float* C, int ldc, int M, int N, int K, const GemmEpilogue& ep,
+              cudaStream_t st) {
+  return profiled(M, N, K, ep, st, [&] { return gemm_nt_impl(A, lda, Bop, C, ldc, M, N, K, ep, st); });
+}
+
+int gemm_nt_planes(const uint16_t* Ahi, const uint16_t* Alo, int ldpa, const BOperand& B, float* C, int ldc, int M, int N, int K,
+                   const GemmEpilogue& ep, cudaStream_t st) {
+  return profiled(M, N, K, ep, st, [&] { return gemm_nt_f16x3_planes(Ahi, Alo, ldpa, B, C, ldc, M, N, K, ep, st); });
 }
 
 }  // namespace mmx

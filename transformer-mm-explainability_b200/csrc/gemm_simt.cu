@@ -100,7 +100,7 @@ __global__ void __launch_bounds__(256) gemm_nt_simt_kernel(const float* __restri
         if (ep.bias) v += ep.bias[gn];
         if (ep.pre) v *= act_bwd(ep.pre[(long long)gm * ep.ldpre + gn], ep.act);
         if (ep.residual) v += ep.residual[(long long)gm * ep.ldres + gn];
-        C[(long long)gm * ldc + gn] = v;
+        if (ep.C_act != C) C[(long long)gm * ldc + gn] = v;
         if (ep.C_act) ep.C_act[(long long)gm * ldc + gn] = act_fwd(v, ep.act);
       }
     }

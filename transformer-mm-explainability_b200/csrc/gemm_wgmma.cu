@@ -293,7 +293,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constan
           const float2 a = *reinterpret_cast<const float2*>(p.ep.residual + r_off + (long long)m * p.ep.ldres + n);
           v.x += a.x; v.y += a.y;
         }
-        *reinterpret_cast<float2*>(p.C + c_off + (long long)m * p.ldc + n) = v;
+        if (!ACT || p.ep.C_act != p.C) *reinterpret_cast<float2*>(p.C + c_off + (long long)m * p.ldc + n) = v;
         if (ACT && p.ep.C_act) *reinterpret_cast<float2*>(p.ep.C_act + (long long)m * p.ldc + n) = act_fwd2(v, p.ep.act);
       }
     }
@@ -423,6 +423,12 @@ static int launch(const Operands& o, const Params& p, cudaStream_t st) {
   }
 }
 
+// the TMA -> wgmma kernel on A already split into fp16 hi / lo' planes [M, ldpa]
+static int gemm_planes(const __half* Ahi, const __half* Alo, int ldpa, const BOperand& B, const Params& p, cudaStream_t st) {
+  const Operands o{Ahi, Alo, ldpa, p.M, B.hi, B.lo, B.ldp, p.N};
+  return launch<F16X3_PRESPLIT>(o, p, st);
+}
+
 // split A once (stream-ordered scratch, same bytes as the fp32 original), then the TMA -> wgmma kernel on the planes
 static int gemm_presplit(const float* A, int lda, const BOperand& B, const Params& p, cudaStream_t st) {
   const int M = p.M, K = p.K, ldpa = round_up(K, 8);
@@ -434,8 +440,7 @@ static int gemm_presplit(const float* A, int lda, const BOperand& B, const Param
   const int grid = (int)((total + 255) / 256 < (long long)sm_count() * 8 ? (total + 255) / 256 : (long long)sm_count() * 8);
   split_a_planes_kernel<<<grid, 256, 0, st>>>(A, lda, Ahi, Alo, ldpa, M, K);
   MMX_LAUNCH_CHECK();
-  const Operands o{Ahi, Alo, ldpa, M, B.hi, B.lo, B.ldp, p.N};
-  const int rc = launch<F16X3_PRESPLIT>(o, p, st);
+  const int rc = gemm_planes(Ahi, Alo, ldpa, B, p, st);
   cudaFreeAsync(planes, st);
   return rc;
 }
@@ -542,15 +547,21 @@ BOperand packed_operand(const float* W, int ldw, const void* packed, int N, int 
   return B;
 }
 
-// Which problems go to the fp16x3 kernels.  Independent of M (a sample alone and inside a batch take the same arithmetic path).
-bool gemm_f16x3_shape_ok(const float* A, int lda, const BOperand& B, float* C, int ldc, int N, int K, const GemmEpilogue& ep) {
+// The part of the fp16x3 rule that does not depend on how A arrives (fp32, or already split into planes): the packed B,
+// the output, the epilogue operands and the tile minimums.
+static bool f16x3_b_epilogue_ok(const BOperand& B, float* C, int ldc, int N, int K, const GemmEpilogue& ep) {
   if (!gemm_tc_available() || !B.hi || !B.lo) return false;
-  if (N < 128 || K < 64 || (N % 4) || (lda % 4) || (B.ldp % 8) || (ldc % 4)) return false;   // K itself is free: TMA zero-fills the tail
-  if (!aligned16(A) || !aligned16(B.hi) || !aligned16(B.lo) || !aligned16(C)) return false;
+  if (N < 128 || K < 64 || (N % 4) || (B.ldp % 8) || (ldc % 4)) return false;   // K itself is free: TMA zero-fills the tail
+  if (!aligned16(B.hi) || !aligned16(B.lo) || !aligned16(C)) return false;
   if ((ep.bias && !aligned16(ep.bias)) || (ep.pre && (!aligned16(ep.pre) || ep.ldpre % 4)) ||
       (ep.residual && (!aligned16(ep.residual) || ep.ldres % 4)) || (ep.C_act && !aligned16(ep.C_act)))
     return false;
   return true;
+}
+
+// Which problems go to the fp16x3 kernels.  Independent of M (a sample alone and inside a batch take the same arithmetic path).
+bool gemm_f16x3_shape_ok(const float* A, int lda, const BOperand& B, float* C, int ldc, int N, int K, const GemmEpilogue& ep) {
+  return (lda % 4) == 0 && aligned16(A) && f16x3_b_epilogue_ok(B, C, ldc, N, K, ep);
 }
 
 int gemm_nt_f16x3(const float* A, int lda, const BOperand& B, float* C, int ldc, int M, int N, int K, const GemmEpilogue& ep,
@@ -560,6 +571,17 @@ int gemm_nt_f16x3(const float* A, int lda, const BOperand& B, float* C, int ldc,
   if (presplit) return wg::gemm_presplit(A, lda, B, p, st);
   const wg::Operands o{A, nullptr, lda, M, B.hi, B.lo, B.ldp, N};
   return wg::launch<wg::F16X3>(o, p, st);
+}
+
+bool gemm_f16x3_planes_ok(int ldpa, const BOperand& B, float* C, int ldc, int N, int K, const GemmEpilogue& ep) {
+  return (ldpa % 8) == 0 && ldpa >= K && f16x3_b_epilogue_ok(B, C, ldc, N, K, ep);
+}
+
+int gemm_nt_f16x3_planes(const uint16_t* Ahi, const uint16_t* Alo, int ldpa, const BOperand& B, float* C, int ldc, int M, int N,
+                         int K, const GemmEpilogue& ep, cudaStream_t st) {
+  if (M == 0 || N == 0) return 0;
+  const wg::Params p{M, N, K, ldc, C, ep};
+  return wg::gemm_planes(reinterpret_cast<const __half*>(Ahi), reinterpret_cast<const __half*>(Alo), ldpa, B, p, st);
 }
 
 }  // namespace mmx

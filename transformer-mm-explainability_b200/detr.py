@@ -2,20 +2,53 @@
 reference signature (DETR/modules/ExplanationGenerator.py:142-195) over the libmmx kernels.
 
 ``DetrEngine`` holds the DETR transformer + class head (DETR/models/transformer.py, DETR/models/detr.py:46-77) built
-from a reference / official-checkpoint ``state_dict`` and runs on backbone features: ``img`` is ``(src, pos)`` with
-``src`` [B, d_model, h, w] (after ``input_proj``) and ``pos`` the sine embedding [B or 1, d_model, h, w].  The ResNet
-backbone sits below every attention layer (no gradient needed) and is outside the hot-path scope of this round.
+from a reference / official-checkpoint ``state_dict``.  ``img`` takes every form ``DETR.forward`` takes
+(DETR/models/detr.py:61-62, DETR/util/misc.py:306-327) when the state dict carries the ResNet backbone
+(``backbone.0.body.*``, ``input_proj.*``; see ``mmx_b200.backbone``):
+
+* a [B, 3, H, W] image tensor (no padding),
+* a list of [3, H_i, W_i] images (zero-padded to the largest H and W, the padding masked),
+* a ``NestedTensor`` (anything with ``.tensors`` / ``.mask``),
+
+and always the backbone features ``(src, pos)``: ``src`` [B, d_model, h, w] (after ``input_proj``) and ``pos`` the sine
+embedding [B or 1, d_model, h, w].  As in the reference the transformer ignores the mask; only ``pos`` sees it.  The
+backbone runs forward only: gradients and LRP stop at the transformer input, as in the reference.  ``Generator`` and
+``MaskGenerator`` also take the reference ``DETR`` ``nn.Module`` itself (its engine is built once, see ``engine_for``).
 """
 from __future__ import annotations
 
 import ctypes as C
+import weakref
 from typing import Dict, List, Optional
 
 import torch
 
 from ._lib import lib, check, ptr, current_stream, MmxError
-from .nn import fp32_gemms, Tape, Var, Weight, AttnRecord, ACT_RELU, _f32
+from .nn import fp32_gemms, Tape, Var, Weight, AttnRecord, ACT_RELU, ACT_SIGMOID, _f32
+from .backbone import DetrBackbone, has_backbone
 from . import rules
+
+
+
+class _Feats:
+    """Transformer input of one call: x = input_proj(src) and pe = pos, both [B*S, d] (row = b*S + y*w + x)."""
+    __slots__ = ("x", "pe", "B", "h", "w", "mask")
+
+    def __init__(self, x, pe, B, h, w, mask=None):
+        self.x, self.pe, self.B, self.h, self.w, self.mask = x, pe, B, h, w, mask
+
+    def expand(self, K: int) -> "_Feats":
+        """the features of one image repeated for K samples (one per query of MaskGenerator)"""
+        assert self.B == 1
+        return _Feats(self.x.repeat(K, 1), self.pe.repeat(K, 1), K, self.h, self.w,
+                      None if self.mask is None else self.mask.expand(K, -1, -1))
+
+
+def _is_features(img) -> bool:
+    """(src [B,d,h,w], pos [B or 1,d,h,w] or [d,h,w]): the feature form the engine has always taken.  Image lists hold
+    [3,H,W] tensors, so a 4-D first element never means an image."""
+    return (isinstance(img, (tuple, list)) and len(img) == 2 and all(isinstance(t, torch.Tensor) for t in img)
+            and img[0].dim() == 4 and img[1].dim() in (3, 4))
 
 
 def _split_mha(sd, p, device):
@@ -40,8 +73,8 @@ class DetrEngine:
         if not torch.cuda.is_available():
             raise MmxError("mmx_b200 needs a CUDA (sm_90a) device; there is no CPU fallback")
         self.device = d = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
-        sd = {(k if k.startswith(("transformer.", "class_embed", "query_embed")) else "transformer." + k): v
-              for k, v in state_dict.items()}
+        sd = {(k if k.startswith(("transformer.", "class_embed", "query_embed", "backbone.", "input_proj.", "bbox_embed."))
+               else "transformer." + k): v for k, v in state_dict.items()}
         self.nhead = nhead
         n_enc = len({k.split(".")[3] for k in sd if k.startswith("transformer.encoder.layers.")})
         n_dec = len({k.split(".")[3] for k in sd if k.startswith("transformer.decoder.layers.")})
@@ -70,12 +103,94 @@ class DetrEngine:
         self.d_model = self.query_embed.shape[1]
         self.queries = self.query_embed.shape[0]
         self.pred_logits: Optional[torch.Tensor] = None
+        self.backbone = DetrBackbone(sd, d) if has_backbone(sd) else None
+        if self.backbone is not None and self.backbone.d_model != self.d_model:
+            raise MmxError(f"input_proj gives {self.backbone.d_model} channels, the transformer takes {self.d_model}")
+        n_box = len({k.split(".")[2] for k in sd if k.startswith("bbox_embed.layers.") and k.endswith(".weight")})
+        self.bbox_embed = [Weight(sd[f"bbox_embed.layers.{i}.weight"], sd[f"bbox_embed.layers.{i}.bias"], d)
+                           for i in range(n_box)]
 
     def eval(self):
         return self
 
     def zero_grad(self):
         return None
+
+    # ------------------------------------------------------------------ inputs
+    def features(self, img) -> _Feats:
+        """The transformer input for any accepted form of ``img`` (module docstring)."""
+        dev = self.device
+        if _is_features(img):
+            src, pos = img
+            B, d, h, w = src.shape
+            if d != self.d_model:
+                raise MmxError(f"src has {d} channels, the transformer takes d_model = {self.d_model} "
+                               "(images go in as a [B,3,H,W] tensor, a list of [3,H,W] tensors or a NestedTensor)")
+            x = _f32(src, dev).flatten(2).permute(0, 2, 1).reshape(B * h * w, d).contiguous()
+            pe = _f32(pos, dev).expand(B, d, h, w).flatten(2).permute(0, 2, 1).reshape(B * h * w, d).contiguous()
+            return _Feats(x, pe, B, h, w)
+        if self.backbone is None:
+            raise MmxError("this DetrEngine was built without backbone weights (backbone.0.body.*, input_proj.*): pass "
+                           "(src, pos) features, or build it from a full DETR state_dict to pass images")
+        images, mask = self._images(img)
+        with torch.cuda.device(dev):
+            x, pe, m, (h, w) = self.backbone(images, mask)
+        return _Feats(x, pe, images.shape[0], h, w, m)
+
+    def _images(self, samples):
+        """(images [B,3,H,W] fp32 on the device, padding mask [B,H,W] or None) as nested_tensor_from_tensor_list builds
+        them (DETR/util/misc.py:306-327)."""
+        dev = self.device
+        if hasattr(samples, "tensors") and hasattr(samples, "mask"):
+            images, mask = samples.tensors, samples.mask
+        elif isinstance(samples, torch.Tensor):
+            if samples.dim() != 4:
+                raise MmxError(f"an image batch is [B, 3, H, W], got {tuple(samples.shape)}")
+            images, mask = samples, None
+        elif isinstance(samples, (list, tuple)) and samples and all(isinstance(t, torch.Tensor) for t in samples):
+            if any(t.dim() != 3 for t in samples):
+                raise MmxError("a list of images holds [3, H, W] tensors")
+            Hm, Wm = max(t.shape[1] for t in samples), max(t.shape[2] for t in samples)
+            images = torch.zeros(len(samples), samples[0].shape[0], Hm, Wm, device=dev, dtype=torch.float32)
+            mask = torch.ones(len(samples), Hm, Wm, device=dev, dtype=torch.bool)
+            for i, t in enumerate(samples):
+                images[i, :, :t.shape[1], :t.shape[2]].copy_(t)
+                mask[i, :t.shape[1], :t.shape[2]] = False
+            if all(t.shape[1:] == (Hm, Wm) for t in samples):
+                mask = None
+        else:
+            raise MmxError("img must be an image tensor [B,3,H,W], a list of [3,H,W] images, a NestedTensor or (src, pos)")
+        if images.dim() != 4 or images.shape[1] != 3:
+            raise MmxError(f"images must have 3 channels ([B, 3, H, W]), got {tuple(images.shape)}")
+        return _f32(images, dev), mask
+
+    # ------------------------------------------------------------------ DETR.forward
+    def forward(self, samples):
+        """``DETR.forward`` (DETR/models/detr.py:46-77): {"pred_logits" [B,Q,C+1], "pred_boxes" [B,Q,4]} of the last decoder
+        layer; pred_boxes = sigmoid(bbox_embed(hs)) (:73, MLP :309-321)."""
+        feats = self.features(samples)
+        self._run(feats, None, backward=False)
+        out = {"pred_logits": self.pred_logits}
+        if self.bbox_embed:
+            out["pred_boxes"] = self._boxes(self.saved["hs"].v)
+        return out
+
+    __call__ = forward
+
+    def _boxes(self, hs: torch.Tensor) -> torch.Tensor:
+        B, S, Q = self._shape
+        l = lib()
+        x = hs
+        with torch.cuda.device(self.device):
+            for i, W in enumerate(self.bbox_embed):
+                last = i == len(self.bbox_embed) - 1
+                y = torch.empty(x.shape[0], W.out_features, device=self.device, dtype=torch.float32)
+                act = ACT_SIGMOID if last else ACT_RELU
+                check(l.mmx_linear_packed(ptr(x), x.stride(0), ptr(W.w), W.in_features, ptr(W.pw), ptr(W.b), None, 0, ptr(y),
+                                          W.out_features, ptr(y), act, x.shape[0], W.out_features, W.in_features,
+                                          current_stream()))
+                x = y
+        return x.view(B, Q, -1)
 
     def _mha(self, tape: Tape, m, query: Var, key: Var, value: Var, B, T, S) -> Var:
         """DETR/modules/layers.py:728-768: separate projections, q scaled before q k^T, masks ignored."""
@@ -86,25 +201,39 @@ class DetrEngine:
         return tape.linear(o, m["o"])
 
     def forward_backward(self, *args, lrp: bool = False, **kwargs):
-        """See ``_forward_backward``.  With ``lrp=True`` every GEMM of the call (forward, dgrad and the relprop sweep) runs
-        on the fp32 FFMA backend (``nn.fp32_gemms``: the sweep amplifies tensor-core split rounding)."""
+        """See ``_forward_backward``.  With ``lrp=True`` every GEMM of the transformer (forward, dgrad and the relprop sweep)
+        runs on the fp32 FFMA backend (``nn.fp32_gemms``: the sweep amplifies tensor-core split rounding); the backbone of
+        an image input runs before that on the default backend - no relevance or gradient reaches it."""
         if lrp:
+            # the backbone sits below the relprop sweep: its features run on the default (tensor-core) backend first
+            if args and not isinstance(args[0], _Feats):
+                pos = args[1] if len(args) > 1 else kwargs.pop("pos", None)
+                feats = self.features(args[0] if pos is None else (args[0], pos))
+                args = (feats, None) + tuple(args[2:])
             with fp32_gemms():
                 return self._forward_backward(*args, lrp=True, **kwargs)
         return self._forward_backward(*args, lrp=False, **kwargs)
 
-    def _forward_backward(self, src: torch.Tensor, pos: torch.Tensor, target_index, index=None, backward: bool = True,
-                         lrp: bool = False):
+    def _forward_backward(self, src, pos=None, target_index=None, index=None, backward: bool = True, lrp: bool = False):
         """Forward staging every A, one-hot on pred_logits[b, target_b, class_b], backward staging every dA
         (``backward=False``: forward only, for the raw-attention / rollout baselines); ``lrp=True`` adds the relprop
-        sweep from the same one-hot (DETR/models/detr.py:79-92), staging the relevance of every A."""
+        sweep from the same one-hot (DETR/models/detr.py:79-92), staging the relevance of every A.  ``src, pos``: the
+        features [B, d, h, w]; or ``src`` alone: any other accepted input (images, ``_Feats``) and ``pos=None``."""
+        if isinstance(src, _Feats):
+            feats = src
+        else:
+            feats = self.features(src if pos is None else (src, pos))
+        return self._run(feats, target_index, index, backward, lrp)
+
+    def _run(self, feats: _Feats, target_index, index=None, backward: bool = True, lrp: bool = False):
         dev = self.device
         with torch.cuda.device(dev):
-            B, d, h, w = src.shape
+            B, h, w, d = feats.B, feats.h, feats.w, self.d_model
             S, Q = h * w, self.queries
+            self.spatial_dim = (h, w)
             tape = Tape(dev)
-            x = Var(_f32(src, dev).flatten(2).permute(0, 2, 1).reshape(B * S, d).contiguous())
-            pe = _f32(pos, dev).expand(B, d, h, w).flatten(2).permute(0, 2, 1).reshape(B * S, d).contiguous()
+            x = Var(feats.x)
+            pe = feats.pe
             qe = self.query_embed.repeat(B, 1)                                    # [B*Q, d]
             for L in self.encoder:                                                # transformer.py:230-254
                 qk = tape.add_const(x, pe)
@@ -156,11 +285,12 @@ class DetrEngine:
 class Generator:
     """DETR/modules/ExplanationGenerator.py:56-195 (``generate_ours`` and its three handlers)."""
 
-    def __init__(self, model: DetrEngine):
-        if not isinstance(model, DetrEngine):
-            raise MmxError("model must be a mmx_b200.DetrEngine")
-        self.model = model
+    def __init__(self, model):
+        self.model = engine_for(model)
         self.model.eval()
+
+    def _feats(self, img) -> _Feats:
+        return img if isinstance(img, _Feats) else self.model.features(img)
 
     def handle_self_attention_image(self, blocks):                                 # :110-118
         for blk in blocks:
@@ -184,9 +314,8 @@ class Generator:
         self.use_lrp = bool(use_lrp)
         self.normalize_self_attention = normalize_self_attention
         self.apply_self_in_rule_10 = apply_self_in_rule_10
-        src, pos = img
         m = self.model
-        m.forward_backward(src, pos, target_index, index, lrp=self.use_lrp)
+        m.forward_backward(self._feats(img), None, target_index, index, lrp=self.use_lrp)
         B, S, Q = m._shape
         self.B = B
         dev = m.device
@@ -211,19 +340,29 @@ class Generator:
 
     def capture(self, img, target_index, index=None, use_lrp=True, normalize_self_attention=True, apply_self_in_rule_10=True):
         """``generate_ours`` for these shapes / flags as a CUDA graph (``mmx_b200.graphs.Graphed``): returns a callable
-        ``g(src, pos, target_index)`` that replays the captured kernels on new inputs and yields the (static) result
+        ``g(src, pos, target_index)`` - or ``g(images, target_index)`` when ``img`` is a [B,3,H,W] image tensor, the
+        backbone then inside the graph - that replays the captured kernels on new inputs and yields the (static) result
         tensor; ``g.check()`` runs the deferred ``diag(R - I) >= 0`` assert.  ``target_index`` must be a tensor."""
         from .graphs import Graphed
-        src, pos = img
         dev = self.model.device
         tq = torch.as_tensor(target_index).reshape(-1).to(dev)
         idx = None if index is None else torch.as_tensor(index).reshape(-1).to(dev)
+        flags = (idx, use_lrp, normalize_self_attention, apply_self_in_rule_10)
+        if _is_features(img):
+            args = (img[0], img[1], tq)
 
-        def fn(s, p, t):
-            return self.generate_ours((s, p), t, idx, use_lrp, normalize_self_attention, apply_self_in_rule_10)
+            def fn(s, p, t):
+                return self.generate_ours((s, p), t, *flags)
+        elif isinstance(img, torch.Tensor):
+            args = (img, tq)
+
+            def fn(x, t):
+                return self.generate_ours(x, t, *flags)
+        else:
+            raise MmxError("capture takes (src, pos) features or a [B,3,H,W] image tensor")
         self._defer_assert = True
         try:
-            return Graphed(fn, (src, pos, tq), dev, deferred_checks=[self.check_min_diag])
+            return Graphed(fn, args, dev, deferred_checks=[self.check_min_diag])
         finally:
             self._defer_assert = False
 
@@ -241,9 +380,8 @@ class Generator:
     # ---- baselines sharing the API (SURVEY.md §8f-2); the LRP ones need relprop and are not implemented
     def generate_raw_attn(self, img, target_index):
         """Head-mean of the last decoder layer's cross-attention (DETR/modules/ExplanationGenerator.py:224-236)."""
-        src, pos = img
         m = self.model
-        m.forward_backward(src, pos, target_index, backward=False)
+        m.forward_backward(self._feats(img), None, target_index, backward=False)
         self.B = m._shape[0]
         self.R_q_i = rules.head_mean_record(m.decoder[-1].multihead_attn["rec"], self.B)
         return self._pick(target_index)
@@ -251,9 +389,8 @@ class Generator:
     def generate_rollout(self, img, target_index):
         """Attention rollout (DETR/modules/ExplanationGenerator.py:238-273): rollout of the encoder and decoder
         self-attentions, combined through the last cross-attention as R_qq^T (A_qi R_ii)."""
-        src, pos = img
         m = self.model
-        m.forward_backward(src, pos, target_index, backward=False)
+        m.forward_backward(self._feats(img), None, target_index, backward=False)
         self.B = B = m._shape[0]
         cams_image = [rules.head_mean_record(blk.self_attn["rec"], B) for blk in m.encoder]
         cams_queries = [rules.head_mean_record(blk.self_attn["rec"], B) for blk in m.decoder]
@@ -266,9 +403,8 @@ class Generator:
 
     def generate_attn_gradcam(self, img, target_index, index=None):
         """attn-GradCAM of the last cross-attention (DETR/modules/ExplanationGenerator.py:275-305)."""
-        src, pos = img
         m = self.model
-        m.forward_backward(src, pos, target_index, index)
+        m.forward_backward(self._feats(img), None, target_index, index)
         self.B = m._shape[0]
         self.R_q_i = rules.gradcam_record(m.decoder[-1].multihead_attn["rec"], self.B)
         return self._pick(target_index)
@@ -276,9 +412,8 @@ class Generator:
     def generate_partial_lrp(self, img, target_index, index=None):
         """Partial LRP (DETR/modules/ExplanationGenerator.py:197-224): head mean of the LRP relevance of the last decoder
         cross-attention, min-max normalised over the whole [Q, S] map."""
-        src, pos = img
         m = self.model
-        m.forward_backward(src, pos, target_index, index, lrp=True)
+        m.forward_backward(self._feats(img), None, target_index, index, lrp=True)
         self.B = B = m._shape[0]
         cam = rules.head_mean_record(m.decoder[-1].multihead_attn["rec"], B, use_cam=True).contiguous()
         self.R_q_i = rules.minmax_normalize(cam)
@@ -287,9 +422,8 @@ class Generator:
     def generate_transformer_att(self, img, target_index, index=None):
         """Transformer attribution (DETR/modules/ExplanationGenerator.py:64-108): rule 5 on the last decoder
         cross-attention with the LRP relevance in place of the probabilities."""
-        src, pos = img
         m = self.model
-        m.forward_backward(src, pos, target_index, index, lrp=True)
+        m.forward_backward(self._feats(img), None, target_index, index, lrp=True)
         self.B = B = m._shape[0]
         self.R_q_i = rules.avg_heads_record(m.decoder[-1].multihead_attn["rec"], B, use_cam=True).contiguous()
         return self._pick(target_index)
@@ -332,20 +466,25 @@ class MaskGenerator:
     METHODS = ("ours_with_lrp", "ours_no_lrp", "ablation_no_self_in_10", "ablation_no_aggregation", "ours_no_lrp_no_norm",
                "transformer_att", "partial_lrp", "raw_attn", "attn_gradcam", "rollout")
 
-    def __init__(self, model: DetrEngine):
+    def __init__(self, model):
         self.gen = Generator(model)
-        self.abl = GeneratorAlbationNoAgg(model)
-        self.model = model
+        self.abl = GeneratorAlbationNoAgg(self.gen.model)
+        self.model = self.gen.model
 
     def get_masks(self, img, queries, method: str = "ours_no_lrp"):
-        """img = (src [1,C,h,w], pos [1,C,h,w]); queries: the kept query indices [K].  Returns (masks [K,h,w] in {0,255},
+        """img: one image (a [1,3,H,W] tensor, a one-image list or NestedTensor) or its features (src [1,C,h,w],
+        pos [1,C,h,w]); queries: the kept query indices [K].  The backbone runs once and its features are repeated over
+        the K queries (the reference re-runs the whole model per query).  Returns (masks [K,h,w] in {0,255},
         thresholds [K], cams [K,h*w])."""
-        src, pos = img
         q = torch.as_tensor(queries).reshape(-1).long()
         K = q.numel()
         if K == 0:
             raise MmxError("no queries to segment")
-        batch = (src.expand(K, *src.shape[1:]).contiguous(), pos.expand(K, *pos.shape[1:]).contiguous())
+        feats = self.model.features(img)
+        if feats.B != 1:
+            raise MmxError(f"get_masks segments one image, got a batch of {feats.B}")
+        batch = feats.expand(K)
+        h, w = feats.h, feats.w
         if method == "ours_no_lrp":
             cam = self.gen.generate_ours(batch, q, use_lrp=False)
         elif method == "ablation_no_self_in_10":
@@ -371,4 +510,27 @@ class MaskGenerator:
             return None
         cam = cam.reshape(K, -1)
         masks, thr = rules.otsu_masks(cam)
-        return masks.view(K, src.shape[-2], src.shape[-1]), thr, cam
+        return masks.view(K, h, w), thr, cam
+
+
+# Engines built from reference ``DETR`` modules, keyed by the module object (dropped with it).  The engine holds a COPY of
+# the weights taken at the first call, like ``mmx_b200.clip.engine_for``.
+_ENGINES: "weakref.WeakKeyDictionary" = weakref.WeakKeyDictionary()
+
+
+def engine_for(model, device=None) -> DetrEngine:
+    """The :class:`DetrEngine` behind ``model``: the engine itself, or one built (once) from a reference ``DETR``
+    ``nn.Module``'s ``state_dict()`` with ``nhead = model.transformer.nhead`` (DETR/models/detr.py:22, transformer.py:42)."""
+    if isinstance(model, DetrEngine):
+        return model
+    if not (hasattr(model, "state_dict") and callable(model.state_dict)):
+        raise MmxError("model must be a mmx_b200.DetrEngine or a reference DETR nn.Module (anything with state_dict())")
+    eng = _ENGINES.get(model)
+    if eng is None:
+        try:
+            nhead = int(model.transformer.nhead)
+        except (AttributeError, TypeError, ValueError):
+            raise MmxError("a DETR module needs model.transformer.nhead (the reference Transformer sets it)") from None
+        eng = DetrEngine(model.state_dict(), nhead=nhead, device=device)
+        _ENGINES[model] = eng
+    return eng

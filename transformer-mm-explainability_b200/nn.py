@@ -18,6 +18,7 @@ import torch
 from ._lib import lib, check, ptr, current_stream, MmxError
 
 ACT_NONE, ACT_QUICKGELU, ACT_GELU, ACT_RELU, ACT_TANH = 0, 1, 2, 3, 4
+ACT_SIGMOID = 6
 ATTN_CAUSAL, ATTN_SCALE_SCORES = 1, 2
 
 
