@@ -229,7 +229,9 @@ int mmx_layernorm_bwd(const float* dy, int lddy, const float* x, int ldx, const 
  * key_bias [B,S] additive or NULL, A [B,H,T,S] row stride ldA, O [B,T,H*hd] (ldo).
  * Replaces the bmm/softmax/bmm of CLIP/clip/auxilary.py:225-252, DETR/modules/layers.py:753-762,
  * lxmert/lxmert/src/lxmert_lrp.py:398-414, including the "save A" hook sites (:247-250 / :758 / :407).
- * hd in {16, 32, 64}; S up to ~1500 keys (score rows live in shared memory).  The products are 3xTF32 tensor-core
+ * hd in {16, 32, 64}; S up to 16384 keys.  Up to 1024 keys (when the score rows of a 32- or 64-query tile fit in shared
+ * memory) one pass per query tile; longer rows run a two-pass kernel (row statistics, then normalised tiles), chosen by
+ * shape alone.  Ragged batches take at most 1024 keys.  The products are 3xTF32 tensor-core
  * passes (error vs fp64 ~1e-6), the softmax is fp32.  A key_bias of -inf REMOVES the key (its probability is exactly 0,
  * the same bits a -10000 mask gives); a row whose keys are all removed gets A = 0 and O = 0 (softmax over an empty set). */
 int mmx_attention_fwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
@@ -261,6 +263,13 @@ int mmx_attention_bwd(const float* dO, int lddo, const float* Q, int ldq, const 
 int mmx_conv2d(const float* x, long long sN, long long sY, long long sX, long long sC, int B, int H, int W, int C,
                const float* Wr, int ldw, const void* packed, const float* bias, const float* residual, int ldres, float* out,
                int ldo, int Cout, int kh, int kw, int stride, int pad, int act, void* stream);
+/* mmx_conv2d with a dilation (F.conv2d(dilation=dilation), DETR's DC5 layer4: torchvision's _make_layer(dilate=True),
+ * DETR/models/backbone.py:88-90): tap (ky, kx) of output pixel (oy, ox) reads input pixel (oy stride - pad + ky dilation,
+ * ox stride - pad + kx dilation), Ho = (H + 2 pad - dilation (kh - 1) - 1) / stride + 1 (same for Wo).  mmx_conv2d is
+ * this entry point with dilation = 1. */
+int mmx_conv2d_dilated(const float* x, long long sN, long long sY, long long sX, long long sC, int B, int H, int W, int C,
+                       const float* Wr, int ldw, const void* packed, const float* bias, const float* residual, int ldres, float* out,
+                       int ldo, int Cout, int kh, int kw, int stride, int pad, int dilation, int act, void* stream);
 /* 3x3 / stride 2 / padding 1 max-pool over NHWC rows (padding acts as -inf, NaN propagates): torchvision ResNet's
  * maxpool (F.max_pool2d).  in: [B*H*W, C] (ldi), out: [B*Ho*Wo, C] (ldo), Ho = (H - 1) / 2 + 1. */
 int mmx_maxpool2d_nhwc(const float* in, int ldi, float* out, int ldo, int B, int H, int W, int C, void* stream);

@@ -106,5 +106,24 @@ for backend in (3, 1):
     l.mmx_set_gemm_backend(backend)
     ieng(ims)
 mmx_b200.Generator(ieng).generate_ours(ims, torch.tensor([0, 1]), use_lrp=False)
+# ---- rows past 1024 keys: the two-pass attention kernels at S = 1100 (forward, backward with dQ / dK / dV, stop after
+# dA, pad columns beyond the last key tile) and dilated convs (the DC5 backbone, fp16 planes and fp32 gathers)
+for hd_ in (16, 32, 64):
+    H_, S_ = 2, 1100
+    D_ = H_ * hd_; ld_ = S_ + 68
+    qkv_ = torch.randn(S_, 3 * D_, device="cuda"); do_ = torch.randn(S_, D_, device="cuda")
+    A_ = torch.empty(1, H_, S_, ld_, device="cuda"); dA_ = torch.empty_like(A_); O_ = torch.empty(S_, D_, device="cuda")
+    dl_ = torch.empty(H_ * S_, device="cuda"); dqkv_ = torch.empty_like(qkv_)
+    check(l.mmx_attention_fwd(ptr(qkv_), 3 * D_, ptr(qkv_[:, D_:]), 3 * D_, ptr(qkv_[:, 2 * D_:]), 3 * D_, None, ptr(A_), ld_, ptr(O_), D_,
+                              1, H_, S_, S_, hd_, C.c_float(hd_ ** -0.5), 0, current_stream()))
+    for full in (True, False):
+        check(l.mmx_attention_bwd(ptr(do_), D_, ptr(qkv_), 3 * D_, ptr(qkv_[:, D_:]), 3 * D_, ptr(qkv_[:, 2 * D_:]), 3 * D_, ptr(A_),
+                                  ptr(dA_), ld_, ptr(dl_) if full else None, ptr(dqkv_) if full else None, 3 * D_,
+                                  ptr(dqkv_[:, D_:]) if full else None, 3 * D_, ptr(dqkv_[:, 2 * D_:]) if full else None, 3 * D_,
+                                  1, H_, S_, S_, hd_, C.c_float(hd_ ** -0.5), 0, current_stream()))
+deng = mmx_b200.DetrEngine(dbo.init_state_dict(dbo.DETR_IMAGE, 3), nhead=dbo.DETR_IMAGE.nhead, device="cuda:0", dilation=True)
+for backend in (3, 1):
+    l.mmx_set_gemm_backend(backend)
+    deng(ims)
 torch.cuda.synchronize()
 print("sanitize_run: all kernels executed")

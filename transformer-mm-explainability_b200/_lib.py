@@ -103,6 +103,9 @@ _SIGS = {
     "mmx_conv2d": (C.c_int, [c_float_p] + [C.c_longlong] * 4 + [C.c_int] * 4 + [c_float_p, C.c_int, C.c_void_p, c_float_p,
                                                                               c_float_p, C.c_int, c_float_p, C.c_int]
                    + [C.c_int] * 6 + [C.c_void_p]),
+    "mmx_conv2d_dilated": (C.c_int, [c_float_p] + [C.c_longlong] * 4 + [C.c_int] * 4 + [c_float_p, C.c_int, C.c_void_p, c_float_p,
+                                                                                      c_float_p, C.c_int, c_float_p, C.c_int]
+                           + [C.c_int] * 7 + [C.c_void_p]),
     "mmx_maxpool2d_nhwc": (C.c_int, [c_float_p, C.c_int, c_float_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "mmx_detr_position_sine": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, c_float_p,
                                          C.c_int, C.c_void_p, C.c_void_p]),

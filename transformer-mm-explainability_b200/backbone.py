@@ -7,8 +7,10 @@ sine position embedding that ``DETR.forward`` runs before the transformer (DETR/
   folded into the conv before it, and each weight is reordered from [Cout, Cin, kh, kw] to [Cout, kh*kw*Cin] (the
   (ky, kx, c) order of the gathered patches) and packed once for the fp16x3 tensor-core GEMM;
 * the bottlenecks follow torchvision's ResNet v1.5 (stride on the 3x3 conv, downsample = 1x1 stride-s conv + BN); the
-  block counts come from the keys (3/4/6/3 for ResNet-50, 3/4/23/3 for ResNet-101).  Dilated layer4 (DC5) checkpoints
-  are not supported: dilation is not visible in the weights, and their 50x50-token maps exceed the attention kernels;
+  block counts come from the keys (3/4/6/3 for ResNet-50, 3/4/23/3 for ResNet-101).  ``dilation=True`` builds the DC5
+  body (DETR/models/backbone.py:88-90, ``--dilation``): layer4 as torchvision's ``_make_layer(dilate=True)``, i.e. block 0
+  with stride 1 (conv2 dilation 1, padding 1, downsample stride 1) and blocks 1.. with conv2 dilation 2, padding 2, so
+  the feature map has stride 16 instead of 32.  Dilation is not visible in the weights: the caller says which it is;
 * activations are NHWC matrices [B*H*W, C].  Convs with fewer than 128 output channels (the stem, layer1's conv1 / conv2,
   an input_proj below 128) are padded to 128 zero rows with zero bias, so every conv meets the tensor-core GEMM's
   N >= 128 rule; their outputs keep a row stride of 128 and consumers read the real channels at that stride.
@@ -58,9 +60,10 @@ class _Act:
 class Conv:
     """One conv (+ folded BN): reordered [rows, kh*kw*Cin] weight padded to >= 128 rows, its bias and packed planes."""
 
-    def __init__(self, w: torch.Tensor, b: Optional[torch.Tensor], stride: int, pad: int, device):
+    def __init__(self, w: torch.Tensor, b: Optional[torch.Tensor], stride: int, pad: int, device, dilation: int = 1):
         cout, cin, kh, kw = w.shape
         self.cout, self.cin, self.kh, self.kw, self.stride, self.pad = cout, cin, kh, kw, stride, pad
+        self.dilation = dilation
         self.rows = max(cout, MIN_ROWS)
         wr = torch.zeros(self.rows, kh * kw * cin, dtype=torch.float32)
         wr[:cout] = w.detach().float().permute(0, 2, 3, 1).reshape(cout, -1).cpu()
@@ -72,15 +75,17 @@ class Conv:
         self.pw = pack_weight(self.w)
 
     def out_hw(self, H, W):
-        return (H + 2 * self.pad - self.kh) // self.stride + 1, (W + 2 * self.pad - self.kw) // self.stride + 1
+        d = self.dilation
+        return ((H + 2 * self.pad - d * (self.kh - 1) - 1) // self.stride + 1,
+                (W + 2 * self.pad - d * (self.kw - 1) - 1) // self.stride + 1)
 
     def __call__(self, x, strides, B, H, W, act=ACT_NONE, residual: Optional[_Act] = None) -> _Act:
         Ho, Wo = self.out_hw(H, W)
         out = torch.empty(B * Ho * Wo, self.rows, device=self.w.device, dtype=torch.float32)
         res = residual.t if residual is not None else None
-        check(lib().mmx_conv2d(ptr(x), *strides, B, H, W, self.cin, ptr(self.w), self.w.stride(0), ptr(self.pw), ptr(self.b),
-                               ptr(res), 0 if res is None else res.stride(0), ptr(out), self.rows, self.rows, self.kh, self.kw,
-                               self.stride, self.pad, act, current_stream()))
+        check(lib().mmx_conv2d_dilated(ptr(x), *strides, B, H, W, self.cin, ptr(self.w), self.w.stride(0), ptr(self.pw),
+                                       ptr(self.b), ptr(res), 0 if res is None else res.stride(0), ptr(out), self.rows, self.rows,
+                                       self.kh, self.kw, self.stride, self.pad, self.dilation, act, current_stream()))
         return _Act(out, B, Ho, Wo, self.cout)
 
     def on(self, a: _Act, act=ACT_NONE, residual: Optional[_Act] = None) -> _Act:
@@ -89,11 +94,13 @@ class Conv:
 
 
 class Bottleneck:
-    """torchvision ResNet v1.5 bottleneck: relu(bn3(conv3(relu(bn2(conv2(relu(bn1(conv1 x)))))) + downsample(x))."""
+    """torchvision ResNet v1.5 bottleneck: relu(bn3(conv3(relu(bn2(conv2(relu(bn1(conv1 x)))))) + downsample(x)); conv2 is
+    the 3x3 conv with padding = dilation."""
 
-    def __init__(self, sd, p, stride, device):
-        conv = lambda n, s, pad: Conv(*fold_frozen_bn(sd[p + f"conv{n}.weight"], _bn(sd, p + f"bn{n}.")), s, pad, device)
-        self.conv1, self.conv2, self.conv3 = conv(1, 1, 0), conv(2, stride, 1), conv(3, 1, 0)
+    def __init__(self, sd, p, stride, device, dilation: int = 1):
+        conv = lambda n, s, pad, dil=1: Conv(*fold_frozen_bn(sd[p + f"conv{n}.weight"], _bn(sd, p + f"bn{n}.")), s, pad, device,
+                                             dil)
+        self.conv1, self.conv2, self.conv3 = conv(1, 1, 0), conv(2, stride, dilation, dilation), conv(3, 1, 0)
         self.down = None
         if p + "downsample.0.weight" in sd:
             self.down = Conv(*fold_frozen_bn(sd[p + "downsample.0.weight"], _bn(sd, p + "downsample.1.")), stride, 0, device)
@@ -110,19 +117,24 @@ def _bn(sd, p):
 
 class DetrBackbone:
     """``backbone(samples)`` -> ``input_proj(src)`` and ``pos`` of DETR.forward (DETR/models/detr.py:63-69), both
-    [B*h*w, d_model] (row = b*h*w + y*w + x), plus the feature-resolution padding mask [B, h, w]."""
+    [B*h*w, d_model] (row = b*h*w + y*w + x), plus the feature-resolution padding mask [B, h, w].  ``dilation=True``: the
+    DC5 body (stride-16 layer4, module docstring)."""
 
-    def __init__(self, state_dict: Dict[str, torch.Tensor], device, temperature: float = 10000.0):
+    def __init__(self, state_dict: Dict[str, torch.Tensor], device, temperature: float = 10000.0, *, dilation: bool = False):
         sd = {k: v for k, v in state_dict.items() if k.startswith((BODY, "input_proj."))}
         sd = {(k[len(BODY):] if k.startswith(BODY) else k): v.detach().to(device) for k, v in sd.items()}
         self.device = torch.device(device)
         self.temperature = temperature
+        self.dilation = bool(dilation)
         self.stem = Conv(*fold_frozen_bn(sd["conv1.weight"], _bn(sd, "bn1.")), 2, 3, device)
         self.layers = []
         for li in range(1, 5):
             idx = sorted({int(m.group(1)) for k in sd for m in [re.match(rf"layer{li}\.(\d+)\.", k)] if m})
             if not idx:
                 raise MmxError(f"state_dict has no {BODY}layer{li}.* keys")
+            if li == 4 and self.dilation:      # _make_layer(dilate=True): stride 1; blocks after the first dilate by 2
+                self.layers.append([Bottleneck(sd, f"layer4.{i}.", 1, device, 1 if i == 0 else 2) for i in idx])
+                continue
             self.layers.append([Bottleneck(sd, f"layer{li}.{i}.", (1 if li == 1 else 2) if i == 0 else 1, device)
                                 for i in idx])
         if "input_proj.weight" not in sd:

@@ -19,7 +19,8 @@
 // element), stages A with coalesced 8-byte stores and leaves the probabilities in shared memory as fp16 planes for P.V.
 //
 // One CTA = one (batch, head, TQ-query tile), TQ/8 warps; the score rows of the tile live in shared memory, so any S up
-// to ~700 (TQ = 64) / ~1024 (TQ = 32: DETR at 800x1066 has 850 keys) is handled without a second pass.  wgmma is
+// to ~700 (TQ = 64) / ~1024 (TQ = 32: DETR at 800x1066 has 850 keys) is handled without a second pass; longer rows (up
+// to 16384 keys) run the two-pass kernels below (attention_fwd_long_kernel / attention_bwd_q_long_kernel).  wgmma is
 // the wrong tool for CLIP ViT-B/32 (a head is 50x50x64, below one 128-row GEMM tile).  Deterministic (no atomics):
 // dK / dV come from a second kernel that walks the query tiles for one key tile.
 #include "mmx_common.cuh"
@@ -727,6 +728,388 @@ __global__ void __launch_bounds__(KV_THREADS) attention_bwd_kv_kernel(
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Long rows: the shapes the single-pass kernels reject (S > 1024, or score rows of a tile beyond shared memory; DETR's
+// DC5 maps have 2500 - 4200 keys).  Nothing holds a whole score row: one CTA = one (b, h, 64-query tile), 8 warps, and
+// the keys stream through shared memory TWICE as 64-key tiles in one cp.async ring (pass-1 tiles, then pass-2 tiles, so
+// the first pass-2 tiles land while pass 1 finishes).  Warp w computes the 16x32 block (rows (w % 4) * 16, keys
+// (w / 4) * 32) of every 64x64 score tile in registers with the same fp16x3 mma.sync products as the short kernels.
+//   forward   pass 1: running row max and sum of exp (per-thread online rescale, combined across the quad and the two
+//                     key halves at the end; fixed order, deterministic);
+//             pass 2: recompute each score tile, normalise, write the A tile (through shared memory: 256-byte row
+//                     stores) and accumulate O += P.V on the probability planes.
+//   backward  pass 1: dA = dO.V^T tile, staged (divided by gscale), delta = rowsum(dA (.) A) from the staged A;
+//             pass 2: re-read A / dA (each thread reads back what it wrote), dS = A (.) (dA - delta), dQ += scale dS.K.
+// The score tile is recomputed instead of stored, so the bound is the A / dA plane traffic (8 bytes per element written
+// or read per pass), not the products.  Plane offsets are 64-bit (B*H*T*ld passes 2^31 at B = 16, S = 4200).
+constexpr int LTQ = 64, LONG_THREADS = 256, LONG_MAX_S = 16384;
+constexpr int LDT = TKEY + 4;     // floats per row of the fp32 tile (16-byte aligned rows)
+constexpr int LDT16 = TKEY + 8;   // halves per row of a probability / dS plane tile (144 bytes: conflict-free ldmatrix)
+
+template <int HD>
+struct LongSmem {
+  static constexpr int LDH = HD + 8, ST = AttnSmem<HD>::STAGE;   // one K or V tile as hi + lo planes
+  // fp32 tile + row statistics, X (Q or dO) planes, P / dS planes, NS ring stages of `per_stage` tiles
+  static size_t bytes(int NS, int per_stage) {
+    return sizeof(float) * ((size_t)LTQ * LDT + 4 * LTQ) +
+           sizeof(__half) * (2 * (size_t)LTQ * LDH + 2 * (size_t)LTQ * LDT16 + (size_t)NS * per_stage * ST);
+  }
+};
+
+// Item `it` of the two-pass key stream into ring stage it % NS (stage stride `sstride` halves): it < nkt -> key tile it
+// of P1; nkt <= it < nit -> key tile it - nkt of P2 (and of P3, into the second half of the stage, when P3h != nullptr).
+// One commit group per item, empty past the end.
+template <int HD>
+__device__ __forceinline__ void issue_stream(const __half* __restrict__ P1h, const __half* __restrict__ P1l, const __half* __restrict__ P2h,
+                                             const __half* __restrict__ P2l, const __half* __restrict__ P3h, const __half* __restrict__ P3l,
+                                             int ldp, long long base, int it, int nkt, int nit, int S, __half* sKV, int NS, int sstride) {
+  constexpr int LDH = HD + 8;
+  if (it < nit) {
+    __half* st = sKV + (size_t)(it % NS) * sstride;
+    if (it < nkt) {
+      load_planes_async<HD, TKEY>(P1h, P1l, ldp, base, it * TKEY, S, st, st + TKEY * LDH);
+    } else {
+      load_planes_async<HD, TKEY>(P2h, P2l, ldp, base, (it - nkt) * TKEY, S, st, st + TKEY * LDH);
+      if (P3h != nullptr) {
+        __half* s3 = st + AttnSmem<HD>::STAGE;
+        load_planes_async<HD, TKEY>(P3h, P3l, ldp, base, (it - nkt) * TKEY, S, s3, s3 + TKEY * LDH);
+      }
+    }
+  }
+  cp_async_commit();
+}
+
+// The warp's 16x32 block of one 64x64 score tile: s[nt][c] = sum_d X[m0 + g + 8 (c >> 1)][d] * Y[kh + 8 nt + 2t + (c & 1)][d]
+template <int HD>
+__device__ __forceinline__ void score_block(const __half* sXh, const __half* sXl, const __half* sYh, const __half* sYl, int m0, int kh,
+                                            int lane, float (&s)[4][4]) {
+  constexpr int LDH = HD + 8;
+  float crs[4][4];
+#pragma unroll
+  for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) s[nt][c] = crs[nt][c] = 0.f;
+#pragma unroll
+  for (int k0 = 0; k0 < HD; k0 += 16) {
+    uint32_t ahi[4], alo[4];
+    ldsm_x4(ahi, addr_a(sXh, LDH, m0, k0, lane));
+    ldsm_x4(alo, addr_a(sXl, LDH, m0, k0, lane));
+#pragma unroll
+    for (int np = 0; np < 2; ++np) {
+      uint32_t bhi[4], blo[4];
+      ldsm_x4(bhi, addr_b2(sYh, LDH, kh + np * 16, k0, lane));
+      ldsm_x4(blo, addr_b2(sYl, LDH, kh + np * 16, k0, lane));
+      mma3(s[2 * np], crs[2 * np], ahi, alo, bhi, blo);
+      mma3(s[2 * np + 1], crs[2 * np + 1], ahi, alo, bhi + 2, blo + 2);
+    }
+  }
+#pragma unroll
+  for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) s[nt][c] = fmaf(crs[nt][c], LO_INV, s[nt][c]);
+}
+
+// out[HD/16][4] (+ crs) += P.Y over one 64-key tile: P as planes [row][key] (LDT16), Y tile [key][d] as planes (transposed
+// on load).  Warp w: rows (w % 4) * 16, d half w / 4.  Keys jn .. 63 are zero in both operands and skipped.  The main
+// products of the tile are summed in their own accumulator and added to `out` once: over thousands of keys a single fp32
+// accumulator would grow its rounding error with sqrt(S) relative to the (1/sqrt(S)-sized) output.
+template <int HD>
+__device__ __forceinline__ void pv_block(const __half* sPh, const __half* sPl, const __half* sYh, const __half* sYl, int m0, int d0,
+                                         int jn, int lane, float (&out)[HD / 16][4], float (&crs)[HD / 16][4]) {
+  constexpr int LDH = HD + 8, NT = HD / 16;
+  float acc[NT][4];
+#pragma unroll
+  for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) acc[nt][c] = 0.f;
+  for (int kk = 0; kk < jn; kk += 16) {
+    uint32_t ahi[4], alo[4];
+    ldsm_x4(ahi, addr_a(sPh, LDT16, m0, kk, lane));
+    ldsm_x4(alo, addr_a(sPl, LDT16, m0, kk, lane));
+    if constexpr (NT >= 2) {
+#pragma unroll
+      for (int np = 0; np < NT / 2; ++np) {
+        uint32_t bhi[4], blo[4];
+        ldsm_x4_t(bhi, addr_bt2(sYh, LDH, kk, d0 + np * 16, lane));
+        ldsm_x4_t(blo, addr_bt2(sYl, LDH, kk, d0 + np * 16, lane));
+        mma3(acc[2 * np], crs[2 * np], ahi, alo, bhi, blo);
+        mma3(acc[2 * np + 1], crs[2 * np + 1], ahi, alo, bhi + 2, blo + 2);
+      }
+    } else {
+      uint32_t bhi[2], blo[2];
+      ldsm_x2_t(bhi, addr_bt2(sYh, LDH, kk, d0, lane & 15));
+      ldsm_x2_t(blo, addr_bt2(sYl, LDH, kk, d0, lane & 15));
+      mma3(acc[0], crs[0], ahi, alo, bhi, blo);
+    }
+  }
+#pragma unroll
+  for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) out[nt][c] += acc[nt][c];
+}
+
+// (m, s) <- the combination of two partial softmax statistics; -inf maxima (every key masked so far) contribute nothing
+__device__ __forceinline__ void merge_stats(float& m, float& s, float m2, float s2) {
+  const float M = fmaxf(m, m2), mref = M == -CUDART_INF_F ? 0.f : M;
+  s = s * expf(m - mref) + s2 * expf(m2 - mref);
+  m = M;
+}
+
+template <int HD, int NS>
+__global__ void __launch_bounds__(LONG_THREADS, HD <= 32 ? 2 : 1) attention_fwd_long_kernel(
+    const __half* __restrict__ Qh, const __half* __restrict__ Ql, const __half* __restrict__ Kh, const __half* __restrict__ Kl,
+    const __half* __restrict__ Vh, const __half* __restrict__ Vl, int ldp, const float* __restrict__ key_bias, float* __restrict__ A,
+    int ldA, float* __restrict__ O, int ldo, int H, int T, int S, float post_scale, int flags) {
+  constexpr int LDH = HD + 8, MB = LTQ / 16, ST = AttnSmem<HD>::STAGE, NT = HD / 16;
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  float* sT = reinterpret_cast<float*>(smem_raw);                 // [LTQ][LDT] normalised probabilities of the tile
+  float* sStat = sT + LTQ * LDT;                                  // [key half][max, sum][LTQ]
+  __half* sXh = reinterpret_cast<__half*>(sStat + 4 * LTQ);
+  __half* sXl = sXh + LTQ * LDH;
+  __half* sPh = sXl + LTQ * LDH;                                  // [LTQ][LDT16] probability planes
+  __half* sPl = sPh + LTQ * LDT16;
+  __half* sKV = sPl + LTQ * LDT16;                                // NS stages of (K tile, V tile) planes
+  const int b = blockIdx.z, h = blockIdx.y, i0 = blockIdx.x * LTQ;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
+  const int m0 = (warp % MB) * 16, kh = (warp / MB) * 32, d0 = (warp / MB) * (HD / 2);
+  const long long kbase = (long long)b * S * ldp + h * HD, plane = ((long long)b * H + h) * T;
+  const int nkt = cdiv(S, TKEY), nit = 2 * nkt;
+  pdl_wait();
+  load_planes_async<HD, LTQ>(Qh, Ql, ldp, (long long)b * T * ldp + h * HD, i0, T, sXh, sXl);   // shares tile 0's group
+#pragma unroll
+  for (int pt = 0; pt < NS - 1; ++pt) issue_stream<HD>(Kh, Kl, Kh, Kl, Vh, Vl, ldp, kbase, pt, nkt, nit, S, sKV, NS, 2 * ST);
+  // score (row m0 + g + 8 (c >> 1), key j0 + kh + 8 nt + 2t + (c & 1)) with the short kernel's order: scale, bias, masks
+  auto finish_scores = [&](float (&s)[4][4], int j0) {
+#pragma unroll
+    for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        const int i = i0 + m0 + g + 8 * (c >> 1), j = j0 + kh + 8 * nt + 2 * t + (c & 1);
+        float v = s[nt][c] * post_scale;
+        if (j >= S) v = -CUDART_INF_F;
+        else {
+          if (key_bias) v += key_bias[(long long)b * S + j];
+          if ((flags & MMX_ATTN_CAUSAL) && j > i) v = -CUDART_INF_F;
+        }
+        s[nt][c] = v;
+      }
+  };
+  // ---- pass 1: row statistics (rows m0 + g and m0 + g + 8 of this thread, over its 8 keys of each tile)
+  float mrun[2] = {-CUDART_INF_F, -CUDART_INF_F}, srun[2] = {0.f, 0.f};
+  for (int it = 0; it < nkt; ++it) {
+    issue_stream<HD>(Kh, Kl, Kh, Kl, Vh, Vl, ldp, kbase, it + NS - 1, nkt, nit, S, sKV, NS, 2 * ST);
+    cp_async_wait<NS - 1>();
+    __syncthreads();
+    const __half* sYh = sKV + (size_t)(it % NS) * 2 * ST;
+    float s[4][4];
+    score_block<HD>(sXh, sXl, sYh, sYh + TKEY * LDH, m0, kh, lane, s);
+    finish_scores(s, it * TKEY);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      float tm = -CUDART_INF_F;
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt) tm = fmaxf(tm, fmaxf(s[nt][2 * r], s[nt][2 * r + 1]));
+      const float M = fmaxf(mrun[r], tm), mref = M == -CUDART_INF_F ? 0.f : M;
+      float acc = srun[r] * expf(mrun[r] - mref);
+#pragma unroll
+      for (int nt = 0; nt < 4; ++nt) acc += expf(s[nt][2 * r] - mref) + expf(s[nt][2 * r + 1] - mref);
+      srun[r] = acc;
+      mrun[r] = M;
+    }
+    __syncthreads();                                  // the stage is refilled in the next iteration
+  }
+  // across the quad (commutative pairwise merges: all four lanes end with the same bits), then across the key halves
+#pragma unroll
+  for (int o = 1; o <= 2; o <<= 1)
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const float m2 = __shfl_xor_sync(0xffffffffu, mrun[r], o), s2 = __shfl_xor_sync(0xffffffffu, srun[r], o);
+      merge_stats(mrun[r], srun[r], m2, s2);
+    }
+  if (t == 0) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      sStat[(warp / MB) * 2 * LTQ + m0 + g + 8 * r] = mrun[r];
+      sStat[(warp / MB) * 2 * LTQ + LTQ + m0 + g + 8 * r] = srun[r];
+    }
+  }
+  __syncthreads();
+  float mref[2], inv[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int row = m0 + g + 8 * r;
+    float m = sStat[row], sum = sStat[LTQ + row];
+    merge_stats(m, sum, sStat[2 * LTQ + row], sStat[3 * LTQ + row]);
+    mref[r] = m == -CUDART_INF_F ? 0.f : m;
+    inv[r] = sum > 0.f ? 1.f / sum : 0.f;            // a row whose keys are all removed: A = 0, output 0
+  }
+  // ---- pass 2: normalised tiles -> A (staged) and the probability planes -> O += P.V
+  float out[NT][4], crs[NT][4];
+#pragma unroll
+  for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) out[nt][c] = crs[nt][c] = 0.f;
+  for (int it = nkt; it < nit; ++it) {
+    issue_stream<HD>(Kh, Kl, Kh, Kl, Vh, Vl, ldp, kbase, it + NS - 1, nkt, nit, S, sKV, NS, 2 * ST);
+    cp_async_wait<NS - 1>();
+    __syncthreads();
+    const __half* sYh = sKV + (size_t)(it % NS) * 2 * ST;
+    const int j0 = (it - nkt) * TKEY;
+    float s[4][4];
+    score_block<HD>(sXh, sXl, sYh, sYh + TKEY * LDH, m0, kh, lane, s);
+    finish_scores(s, j0);
+#pragma unroll
+    for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const float2 p = make_float2(expf(s[nt][2 * r] - mref[r]) * inv[r], expf(s[nt][2 * r + 1] - mref[r]) * inv[r]);
+        const int row = m0 + g + 8 * r, col = kh + 8 * nt + 2 * t;
+        *reinterpret_cast<float2*>(sT + row * LDT + col) = p;
+        uint32_t ph, pl;
+        split_f16(p.x, p.y, ph, pl);
+        *reinterpret_cast<uint32_t*>(sPh + row * LDT16 + col) = ph;
+        *reinterpret_cast<uint32_t*>(sPl + row * LDT16 + col) = pl;
+      }
+    __syncthreads();
+    for (int e = tid; e < LTQ * (TKEY / 4); e += LONG_THREADS) {     // 16 threads per 256-byte row segment
+      const int r = e / (TKEY / 4), c = (e % (TKEY / 4)) * 4, i = i0 + r, j = j0 + c;
+      if (i < T && j < ldA) *reinterpret_cast<float4*>(A + (plane + i) * ldA + j) = *reinterpret_cast<const float4*>(sT + r * LDT + c);
+    }
+    pv_block<HD>(sPh, sPl, sYh + ST, sYh + ST + TKEY * LDH, m0, d0, min(TKEY, S - j0), lane, out, crs);
+    __syncthreads();                                  // the stage and the tiles are rewritten in the next iteration
+  }
+  const int jz = nkt * TKEY;                          // pad columns the tiles did not reach
+  if (jz < ldA)
+    for (int e = tid; e < LTQ * (ldA - jz); e += LONG_THREADS) {
+      const int i = i0 + e / (ldA - jz);
+      if (i < T) A[(plane + i) * ldA + jz + e % (ldA - jz)] = 0.f;
+    }
+#pragma unroll
+  for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) out[nt][c] = fmaf(crs[nt][c], LO_INV, out[nt][c]);
+  store_pv<HD, MB>(O, ldo, (long long)b * T, i0, T, h, out, 1.f);
+}
+
+template <int HD, int NS>
+__global__ void __launch_bounds__(LONG_THREADS, 2) attention_bwd_q_long_kernel(
+    const __half* __restrict__ Gh, const __half* __restrict__ Gl, int ldg, const __half* __restrict__ Kh, const __half* __restrict__ Kl,
+    const __half* __restrict__ Vh, const __half* __restrict__ Vl, int ldp, const float* __restrict__ A, float* __restrict__ dA, int ldA,
+    float* __restrict__ delta, float* __restrict__ dQ, int lddq, int H, int T, int S, float scale, const float* __restrict__ gscale) {
+  constexpr int LDH = HD + 8, MB = LTQ / 16, ST = AttnSmem<HD>::STAGE, NT = HD / 16, RPW = LTQ / (LONG_THREADS / 32);
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  float* sT = reinterpret_cast<float*>(smem_raw);                 // [LTQ][LDT] dA tile (scaled units)
+  float* sDelta = sT + LTQ * LDT;                                 // [LTQ]
+  __half* sXh = reinterpret_cast<__half*>(sDelta + 4 * LTQ);
+  __half* sXl = sXh + LTQ * LDH;
+  __half* sPh = sXl + LTQ * LDH;                                  // [LTQ][LDT16] dS planes
+  __half* sPl = sPh + LTQ * LDT16;
+  __half* sKV = sPl + LTQ * LDT16;                                // NS stages of one V (pass 1) or K (pass 2) tile
+  const int b = blockIdx.z, h = blockIdx.y, i0 = blockIdx.x * LTQ;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
+  const int m0 = (warp % MB) * 16, kh = (warp / MB) * 32, d0 = (warp / MB) * (HD / 2);
+  const long long kbase = (long long)b * S * ldp + h * HD, plane = ((long long)b * H + h) * T;
+  const int nkt = cdiv(S, TKEY), nit = dQ != nullptr ? 2 * nkt : nkt;
+  pdl_wait();
+  // dA is staged in TRUE units (divided by the power-of-two gscale[b], exact); delta, dS and dQ stay scaled
+  const float gs = gscale ? gscale[b] : 1.f, ginv = gscale ? 1.f / gscale[b] : 1.f;
+  load_planes_async<HD, LTQ>(Gh, Gl, ldg, (long long)b * T * ldg + h * HD, i0, T, sXh, sXl);
+#pragma unroll
+  for (int pt = 0; pt < NS - 1; ++pt) issue_stream<HD>(Vh, Vl, Kh, Kl, nullptr, nullptr, ldp, kbase, pt, nkt, nit, S, sKV, NS, ST);
+  // ---- pass 1: dA tiles -> staged dA, delta.  Warp w owns rows w * RPW .. +RPW-1, lane l the key pair (2l, 2l+1) of a tile.
+  float dl[RPW];
+#pragma unroll
+  for (int u = 0; u < RPW; ++u) dl[u] = 0.f;
+  for (int it = 0; it < nkt; ++it) {
+    issue_stream<HD>(Vh, Vl, Kh, Kl, nullptr, nullptr, ldp, kbase, it + NS - 1, nkt, nit, S, sKV, NS, ST);
+    cp_async_wait<NS - 1>();
+    __syncthreads();
+    const __half* sYh = sKV + (size_t)(it % NS) * ST;
+    const int j0 = it * TKEY;
+    float s[4][4];
+    score_block<HD>(sXh, sXl, sYh, sYh + TKEY * LDH, m0, kh, lane, s);
+#pragma unroll
+    for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int col = kh + 8 * nt + 2 * t;
+        float2 v = make_float2(s[nt][2 * r], s[nt][2 * r + 1]);
+        if (j0 + col >= S) v.x = 0.f;
+        if (j0 + col + 1 >= S) v.y = 0.f;
+        *reinterpret_cast<float2*>(sT + (m0 + g + 8 * r) * LDT + col) = v;
+      }
+    __syncthreads();
+    const int j = j0 + 2 * lane;
+#pragma unroll
+    for (int u = 0; u < RPW; ++u) {
+      const int r = warp * RPW + u, i = i0 + r;
+      if (i < T && j < ldA) {                         // j even, ldA % 4 == 0: the pair is inside the row
+        const float2 gv = *reinterpret_cast<const float2*>(sT + r * LDT + 2 * lane);
+        const long long off = (plane + i) * ldA + j;
+        const float2 av = *reinterpret_cast<const float2*>(A + off);     // pad columns of A are zero
+        *reinterpret_cast<float2*>(dA + off) = make_float2(gv.x * ginv, gv.y * ginv);
+        dl[u] = fmaf(gv.x, av.x, dl[u]);
+        dl[u] = fmaf(gv.y, av.y, dl[u]);
+      }
+    }
+    __syncthreads();                                  // the stage and the tile are rewritten in the next iteration
+  }
+  const int jz = nkt * TKEY;
+#pragma unroll
+  for (int u = 0; u < RPW; ++u) {
+    const int r = warp * RPW + u, i = i0 + r;
+    if (i < T) for (int j = jz + lane; j < ldA; j += 32) dA[(plane + i) * ldA + j] = 0.f;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) dl[u] += __shfl_xor_sync(0xffffffffu, dl[u], o);
+    if (lane == 0) {
+      sDelta[r] = dl[u];
+      if (delta && i < T) delta[plane + i] = dl[u];
+    }
+  }
+  if (dQ == nullptr) return;
+  __syncwarp();                                       // sDelta of the warp's rows is read by every lane below
+  // ---- pass 2: dS = A (.) (dA - delta) planes -> dQ += dS.K
+  float out[NT][4], crs[NT][4];
+#pragma unroll
+  for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) out[nt][c] = crs[nt][c] = 0.f;
+  for (int it = nkt; it < nit; ++it) {
+    issue_stream<HD>(Vh, Vl, Kh, Kl, nullptr, nullptr, ldp, kbase, it + NS - 1, nkt, nit, S, sKV, NS, ST);
+    const int j0 = (it - nkt) * TKEY, j = j0 + 2 * lane;
+    float2 av[RPW], gv[RPW];
+#pragma unroll
+    for (int u = 0; u < RPW; ++u) {                   // the same (row, pair) this thread staged in pass 1
+      const int i = i0 + warp * RPW + u;
+      av[u] = gv[u] = make_float2(0.f, 0.f);
+      if (i < T && j < S) {
+        const long long off = (plane + i) * ldA + j;
+        av[u] = *reinterpret_cast<const float2*>(A + off);
+        gv[u] = *reinterpret_cast<const float2*>(dA + off);
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < RPW; ++u) {
+      const int r = warp * RPW + u;
+      const float dlr = sDelta[r];                    // written by lane 0 of this warp
+      uint32_t sh, sl;
+      split_f16(av[u].x * (gv[u].x * gs - dlr), av[u].y * (gv[u].y * gs - dlr), sh, sl);
+      *reinterpret_cast<uint32_t*>(sPh + r * LDT16 + 2 * lane) = sh;
+      *reinterpret_cast<uint32_t*>(sPl + r * LDT16 + 2 * lane) = sl;
+    }
+    cp_async_wait<NS - 1>();
+    __syncthreads();
+    const __half* sYh = sKV + (size_t)(it % NS) * ST;
+    pv_block<HD>(sPh, sPl, sYh, sYh + TKEY * LDH, m0, d0, min(TKEY, S - j0), lane, out, crs);
+    __syncthreads();
+  }
+#pragma unroll
+  for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) out[nt][c] = fmaf(crs[nt][c], LO_INV, out[nt][c]);
+  store_pv<HD, MB>(dQ, lddq, (long long)b * T, i0, T, h, out, scale);
+}
+
 constexpr size_t ATT_SMEM_MAX = 227 * 1024;
 
 void attention_set_trace(long long* buf) { cudaMemcpyToSymbol(g_attn_trace, &buf, sizeof(buf)); }
@@ -777,14 +1160,43 @@ static int launch_fwd_tq(const __half* Qh, const __half* Ql, const __half* Kh, c
   return 0;
 }
 
+// The single-pass kernels take a shape when a score row fits the registers of a warp (S <= 1024) and the score rows of a
+// 32- or 64-query tile fit in shared memory; every other shape runs the two-pass kernels.
+template <int HD>
+static bool single_pass_ok(int S) {
+  return S <= 64 * MAX_PAIRS && (AttnSmem<HD>::bytes(S, 64) <= ATT_SMEM_MAX || AttnSmem<HD>::bytes(S, 32) <= ATT_SMEM_MAX);
+}
+
+constexpr int LONG_NS = 3;   // ring depth of the two-pass kernels
+
+static int check_long(int S, const Ragged& rg) {
+  MMX_REQUIRE(S <= LONG_MAX_S, "attention: at most 16384 keys per row");
+  MMX_REQUIRE(rg.lens == nullptr, "ragged attention: at most 1024 keys per row");
+  return 0;
+}
+
+template <int HD>
+static int launch_fwd_long(const __half* Qh, const __half* Ql, const __half* Kh, const __half* Kl, const __half* Vh, const __half* Vl,
+                           int ldp, const float* key_bias, float* A, int ldA, float* O, int ldo, int B, int H, int T, int S,
+                           float post, int flags, Ragged rg, cudaStream_t st) {
+  MMX_TRY(check_long(S, rg));
+  MMX_REQUIRE(Ql != nullptr, "long attention takes pre-split planes");
+  const size_t smem = LongSmem<HD>::bytes(LONG_NS, 2);
+  MMX_CHECK_CUDA(cudaFuncSetAttribute(attention_fwd_long_kernel<HD, LONG_NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  dim3 grid(cdiv(T, LTQ), H, B);
+  MMX_CHECK_CUDA(launch_pdl(attention_fwd_long_kernel<HD, LONG_NS>, grid, dim3(LONG_THREADS), smem, st, Qh, Ql, Kh, Kl, Vh, Vl, ldp,
+                            key_bias, A, ldA, O, ldo, H, T, S, post, flags));
+  MMX_LAUNCH_CHECK();
+  return 0;
+}
+
 // forward on ready-made planes (row stride ldp halves; Q already carries the pre-product scale)
 template <int HD>
 static int launch_fwd_planes(const __half* Qh, const __half* Ql, const __half* Kh, const __half* Kl, const __half* Vh, const __half* Vl,
                              int ldp, const float* key_bias, float* A, int ldA, float* O, int ldo, int B, int H, int T, int S,
                              float q_mul, float post, int flags, Ragged rg, cudaStream_t st) {
-  MMX_REQUIRE(S <= 64 * MAX_PAIRS, "attention: at most 1024 keys per row");
+  if (!single_pass_ok<HD>(S)) return launch_fwd_long<HD>(Qh, Ql, Kh, Kl, Vh, Vl, ldp, key_bias, A, ldA, O, ldo, B, H, T, S, post, flags, rg, st);
   const bool tq64 = AttnSmem<HD>::bytes(S, 64) <= ATT_SMEM_MAX;
-  MMX_REQUIRE(tq64 || AttnSmem<HD>::bytes(S, 32) <= ATT_SMEM_MAX, "sequence too long for the single-pass attention kernel");
 #define MMX_FWD(TQ_, NP_, NS_) \
   return launch_fwd_tq<HD, TQ_, NP_, NS_>(Qh, Ql, Kh, Kl, Vh, Vl, ldp, key_bias, A, ldA, O, ldo, B, H, T, S, q_mul, post, flags, rg, st)
   if (S <= 128) MMX_FWD(64, 2, 2);
@@ -847,12 +1259,19 @@ static int launch_bwd_planes(const __half* Gh, const __half* Gl, int ldg, const 
                              const __half* Kl, const __half* Vh, const __half* Vl, int ldp, const float* A, float* dA, int ldA,
                              float* delta, float* dQ, int lddq, float* dK, int lddk, float* dV, int lddv, int B, int H, int T, int S,
                              float scale_q, float scale_k, Ragged rg, const float* gscale, cudaStream_t st) {
-  MMX_REQUIRE(S <= 64 * MAX_PAIRS, "attention: at most 1024 keys per row");
   const bool tq64 = AttnSmem<HD>::bytes(S, 64) <= ATT_SMEM_MAX;
-  MMX_REQUIRE(tq64 || AttnSmem<HD>::bytes(S, 32) <= ATT_SMEM_MAX, "sequence too long for the single-pass attention kernel");
 #define MMX_BWDQ(TQ_, NP_, NS_) \
   MMX_TRY((launch_bwd_q_tq<HD, TQ_, NP_, NS_>(Gh, Gl, ldg, Kh, Kl, Vh, Vl, ldp, A, dA, ldA, delta, dQ, lddq, B, H, T, S, scale_q, rg, gscale, st)))
-  if (S <= 128) {
+  if (!single_pass_ok<HD>(S)) {
+    MMX_TRY(check_long(S, rg));
+    MMX_REQUIRE(Gl != nullptr, "long attention takes pre-split planes");
+    const size_t smem = LongSmem<HD>::bytes(LONG_NS, 1);
+    MMX_CHECK_CUDA(cudaFuncSetAttribute(attention_bwd_q_long_kernel<HD, LONG_NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    dim3 grid(cdiv(T, LTQ), H, B);
+    MMX_CHECK_CUDA(launch_pdl(attention_bwd_q_long_kernel<HD, LONG_NS>, grid, dim3(LONG_THREADS), smem, st, Gh, Gl, ldg, Kh, Kl, Vh, Vl,
+                              ldp, A, dA, ldA, delta, dQ, lddq, H, T, S, scale_q, gscale));
+    MMX_LAUNCH_CHECK();
+  } else if (S <= 128) {
     MMX_BWDQ(64, 2, 2);
   } else if (tq64) {
     switch (pick_stages<HD>(S, 64)) { case 4: MMX_BWDQ(64, MAX_PAIRS, 4); break; case 3: MMX_BWDQ(64, MAX_PAIRS, 3); break; default: MMX_BWDQ(64, MAX_PAIRS, 2); }

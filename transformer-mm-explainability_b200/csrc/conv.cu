@@ -24,10 +24,11 @@ __device__ __forceinline__ void split_pair(float x0, float x1, uint32_t& hi, uin
 
 struct ConvGeom {
   long long sN, sY, sX, sC;
-  int H, W, C, Ho, Wo, kw, stride, pad, M, K;
+  int H, W, C, Ho, Wo, kw, stride, pad, dil, M, K;
 };
 
-// Row m, columns k0 .. k0+3 of the patch matrix (zero outside the image and beyond K).  VEC: C % 4 == 0, sC == 1 and
+// Row m, columns k0 .. k0+3 of the patch matrix (zero outside the image and beyond K); tap (ky, kx) of output pixel
+// (oy, ox) reads input pixel (oy stride - pad + ky dil, ox stride - pad + kx dil), as F.conv2d with dilation = dil.  VEC: C % 4 == 0, sC == 1 and
 // every other stride and the base 16-byte aligned - the four columns are one float4 of one pixel.
 template <bool VEC>
 __device__ __forceinline__ float4 patch4(const float* __restrict__ x, const ConvGeom& g, int m, int k0) {
@@ -36,7 +37,7 @@ __device__ __forceinline__ float4 patch4(const float* __restrict__ x, const Conv
   const float* xb = x + b * g.sN;
   if constexpr (VEC) {
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    const int c = k0 % g.C, t = k0 / g.C, kx = t % g.kw, ky = t / g.kw, iy = iy0 + ky, ix = ix0 + kx;
+    const int c = k0 % g.C, t = k0 / g.C, kx = t % g.kw, ky = t / g.kw, iy = iy0 + ky * g.dil, ix = ix0 + kx * g.dil;
     if (k0 < g.K && iy >= 0 && iy < g.H && ix >= 0 && ix < g.W)
       v = __ldg(reinterpret_cast<const float4*>(xb + iy * g.sY + ix * g.sX + c));
     return v;
@@ -44,7 +45,7 @@ __device__ __forceinline__ float4 patch4(const float* __restrict__ x, const Conv
     float e[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      const int k = k0 + i, c = k % g.C, t = k / g.C, kx = t % g.kw, ky = t / g.kw, iy = iy0 + ky, ix = ix0 + kx;
+      const int k = k0 + i, c = k % g.C, t = k / g.C, kx = t % g.kw, ky = t / g.kw, iy = iy0 + ky * g.dil, ix = ix0 + kx * g.dil;
       e[i] = (k < g.K && iy >= 0 && iy < g.H && ix >= 0 && ix < g.W) ? __ldg(xb + iy * g.sY + ix * g.sX + c * g.sC) : 0.f;
     }
     return make_float4(e[0], e[1], e[2], e[3]);
@@ -156,12 +157,12 @@ int grid_for(long long total) {
 using namespace mmx;
 extern "C" {
 
-int mmx_conv2d(const float* x, long long sN, long long sY, long long sX, long long sC, int B, int H, int W, int C,
-               const float* Wr, int ldw, const void* packed, const float* bias, const float* residual, int ldres, float* out,
-               int ldo, int Cout, int kh, int kw, int stride, int pad, int act, void* stream) {
-  MMX_REQUIRE(x && Wr && out && B > 0 && H > 0 && W > 0 && C > 0 && Cout > 0 && kh > 0 && kw > 0 && stride > 0 && pad >= 0,
-              "bad arguments");
-  const int Ho = (H + 2 * pad - kh) / stride + 1, Wo = (W + 2 * pad - kw) / stride + 1;
+int mmx_conv2d_dilated(const float* x, long long sN, long long sY, long long sX, long long sC, int B, int H, int W, int C,
+                       const float* Wr, int ldw, const void* packed, const float* bias, const float* residual, int ldres, float* out,
+                       int ldo, int Cout, int kh, int kw, int stride, int pad, int dilation, int act, void* stream) {
+  MMX_REQUIRE(x && Wr && out && B > 0 && H > 0 && W > 0 && C > 0 && Cout > 0 && kh > 0 && kw > 0 && stride > 0 && pad >= 0 &&
+              dilation > 0, "bad arguments");
+  const int Ho = (H + 2 * pad - dilation * (kh - 1) - 1) / stride + 1, Wo = (W + 2 * pad - dilation * (kw - 1) - 1) / stride + 1;
   MMX_REQUIRE(Ho > 0 && Wo > 0, "kernel larger than the padded input");
   const long long Ml = (long long)B * Ho * Wo;
   MMX_REQUIRE(Ml < (1ll << 31) && (long long)kh * kw * C < (1 << 30), "problem too large");
@@ -177,7 +178,7 @@ int mmx_conv2d(const float* x, long long sN, long long sY, long long sX, long lo
       sX < (1 << 30))
     return gemm_nt_b(x, (int)sX, Bop, out, ldo, M, Cout, K, ep, st);
   keep_stream_scratch_cached();
-  ConvGeom g{sN, sY, sX, sC, H, W, C, Ho, Wo, kw, stride, pad, M, K};
+  ConvGeom g{sN, sY, sX, sC, H, W, C, Ho, Wo, kw, stride, pad, dilation, M, K};
   const bool vec = C % 4 == 0 && sC == 1 && sN % 4 == 0 && sY % 4 == 0 && sX % 4 == 0 && aligned16(x);
   const long long total = (long long)M * ((K + 3) / 4);
   auto gather = [&](int ld, float* f32, __half* hi, __half* lo) {
@@ -205,6 +206,13 @@ int mmx_conv2d(const float* x, long long sN, long long sY, long long sX, long lo
   const int rc = gemm_nt_b(patches, lda, Bop, out, ldo, M, Cout, K, ep, st);
   cudaFreeAsync(patches, st);
   return rc;
+}
+
+int mmx_conv2d(const float* x, long long sN, long long sY, long long sX, long long sC, int B, int H, int W, int C,
+               const float* Wr, int ldw, const void* packed, const float* bias, const float* residual, int ldres, float* out,
+               int ldo, int Cout, int kh, int kw, int stride, int pad, int act, void* stream) {
+  return mmx_conv2d_dilated(x, sN, sY, sX, sC, B, H, W, C, Wr, ldw, packed, bias, residual, ldres, out, ldo, Cout, kh, kw, stride,
+                            pad, 1, act, stream);
 }
 
 int mmx_maxpool2d_nhwc(const float* in, int ldi, float* out, int ldo, int B, int H, int W, int C, void* stream) {

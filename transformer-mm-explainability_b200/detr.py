@@ -4,7 +4,8 @@ reference signature (DETR/modules/ExplanationGenerator.py:142-195) over the libm
 ``DetrEngine`` holds the DETR transformer + class head (DETR/models/transformer.py, DETR/models/detr.py:46-77) built
 from a reference / official-checkpoint ``state_dict``.  ``img`` takes every form ``DETR.forward`` takes
 (DETR/models/detr.py:61-62, DETR/util/misc.py:306-327) when the state dict carries the ResNet backbone
-(``backbone.0.body.*``, ``input_proj.*``; see ``mmx_b200.backbone``):
+(``backbone.0.body.*``, ``input_proj.*``; see ``mmx_b200.backbone``; ``dilation=True`` for the DC5 checkpoints, whose
+stride-16 maps give 2500 - 4200 tokens at COCO sizes):
 
 * a [B, 3, H, W] image tensor (no padding),
 * a list of [3, H_i, W_i] images (zero-padded to the largest H and W, the padding masked),
@@ -69,7 +70,7 @@ class _Layer:
 
 
 class DetrEngine:
-    def __init__(self, state_dict: Dict[str, torch.Tensor], nhead: int = 8, device=None):
+    def __init__(self, state_dict: Dict[str, torch.Tensor], nhead: int = 8, device=None, dilation: bool = False):
         if not torch.cuda.is_available():
             raise MmxError("mmx_b200 needs a CUDA (sm_90a) device; there is no CPU fallback")
         self.device = d = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
@@ -103,7 +104,8 @@ class DetrEngine:
         self.d_model = self.query_embed.shape[1]
         self.queries = self.query_embed.shape[0]
         self.pred_logits: Optional[torch.Tensor] = None
-        self.backbone = DetrBackbone(sd, d) if has_backbone(sd) else None
+        self.dilation = bool(dilation)
+        self.backbone = DetrBackbone(sd, d, dilation=self.dilation) if has_backbone(sd) else None
         if self.backbone is not None and self.backbone.d_model != self.d_model:
             raise MmxError(f"input_proj gives {self.backbone.d_model} channels, the transformer takes {self.d_model}")
         n_box = len({k.split(".")[2] for k in sd if k.startswith("bbox_embed.layers.") and k.endswith(".weight")})
@@ -461,7 +463,11 @@ class MaskGenerator:
     """The relevance -> segmentation-mask step of DETR/mask_generator.py:39-125 (``get_panoptic``): one relevance map per
     kept query through the ``method`` switch (:93-113), then min-max / Otsu (:115-121).  The reference loops over the
     kept queries with one forward + backward and one CPU cv2 call each; here the queries of an image form ONE batch and
-    the masks come from one kernel launch.  The visualisation / COCO panoptic bookkeeping around it is out of scope."""
+    the masks come from one kernel launch.  The visualisation / COCO panoptic bookkeeping around it is out of scope.
+
+    The staged A / dA of every encoder layer grow with S^2 (about 2.4 GB per query at 2500 tokens, 6.8 GB at 4200), so the
+    queries run in chunks: ``max_batch`` queries per chunk when given, else as many as the free device memory holds
+    (``chunk_size``).  Every query's map is the same bits whatever the chunking (the kernels are batch invariant)."""
 
     METHODS = ("ours_with_lrp", "ours_no_lrp", "ablation_no_self_in_10", "ablation_no_aggregation", "ours_no_lrp_no_norm",
                "transformer_att", "partial_lrp", "raw_attn", "attn_gradcam", "rollout")
@@ -471,20 +477,51 @@ class MaskGenerator:
         self.abl = GeneratorAlbationNoAgg(self.gen.model)
         self.model = self.gen.model
 
-    def get_masks(self, img, queries, method: str = "ours_no_lrp"):
+    def sample_bytes(self, S: int, lrp: bool) -> int:
+        """Device memory one query of a chunk stages at S tokens: A and dA of every attention layer (fp32, rows padded to a
+        multiple of 4), the relevancy matrices (R_i_i, rule 6's product and its operand), and half as much again under LRP
+        (the relevance planes and the sweep's activations)."""
+        m = self.model
+        H, Q, ld = m.nhead, m.queries, -(-S // 4) * 4
+        staged = 2 * H * (len(m.encoder) * S * ld + len(m.decoder) * Q * (ld + Q))
+        rel = 3 * S * S + 2 * Q * S
+        total = 4 * (staged + rel)
+        return total * 3 // 2 if lrp else total
+
+    def chunk_size(self, S: int, lrp: bool, budget: float = 0.7) -> int:
+        """Queries per chunk: ``budget`` of the free device memory (including what PyTorch's allocator holds unused) over
+        ``sample_bytes``, at least 1."""
+        dev = self.model.device
+        free, _ = torch.cuda.mem_get_info(dev)
+        free += torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+        return max(1, int(budget * free) // self.sample_bytes(S, lrp))
+
+    def get_masks(self, img, queries, method: str = "ours_no_lrp", max_batch: Optional[int] = None):
         """img: one image (a [1,3,H,W] tensor, a one-image list or NestedTensor) or its features (src [1,C,h,w],
         pos [1,C,h,w]); queries: the kept query indices [K].  The backbone runs once and its features are repeated over
-        the K queries (the reference re-runs the whole model per query).  Returns (masks [K,h,w] in {0,255},
-        thresholds [K], cams [K,h*w])."""
+        the queries of each chunk (the reference re-runs the whole model per query); ``max_batch`` caps the queries per
+        chunk (default: ``chunk_size``).  Returns (masks [K,h,w] in {0,255}, thresholds [K], cams [K,h*w])."""
         q = torch.as_tensor(queries).reshape(-1).long()
         K = q.numel()
         if K == 0:
             raise MmxError("no queries to segment")
+        if method not in self.METHODS:
+            print("please provide a valid explainability method")            # mask_generator.py:111-113
+            return None
+        if max_batch is not None and int(max_batch) < 1:
+            raise MmxError(f"max_batch must be >= 1, got {max_batch}")
         feats = self.model.features(img)
         if feats.B != 1:
             raise MmxError(f"get_masks segments one image, got a batch of {feats.B}")
-        batch = feats.expand(K)
         h, w = feats.h, feats.w
+        lrp = method in ("ours_with_lrp", "transformer_att", "partial_lrp")
+        n = int(max_batch) if max_batch is not None else self.chunk_size(h * w, lrp)
+        cam = torch.cat([self._cams(feats.expand(len(qc)), qc, method) for qc in q.split(n)])
+        masks, thr = rules.otsu_masks(cam)
+        return masks.view(K, h, w), thr, cam
+
+    def _cams(self, batch: _Feats, q: torch.Tensor, method: str) -> torch.Tensor:
+        """the relevance maps [k, h*w] of the k queries ``q`` (one per sample of ``batch``) by ``method`` (:93-113)"""
         if method == "ours_no_lrp":
             cam = self.gen.generate_ours(batch, q, use_lrp=False)
         elif method == "ablation_no_self_in_10":
@@ -503,14 +540,9 @@ class MaskGenerator:
             cam = self.gen.generate_ours(batch, q, use_lrp=True)
         elif method == "transformer_att":
             cam = self.gen.generate_transformer_att(batch, q)
-        elif method == "partial_lrp":
-            cam = self.gen.generate_partial_lrp(batch, q)
         else:
-            print("please provide a valid explainability method")            # mask_generator.py:111-113
-            return None
-        cam = cam.reshape(K, -1)
-        masks, thr = rules.otsu_masks(cam)
-        return masks.view(K, h, w), thr, cam
+            cam = self.gen.generate_partial_lrp(batch, q)
+        return cam.reshape(q.numel(), -1)
 
 
 # Engines built from reference ``DETR`` modules, keyed by the module object (dropped with it).  The engine holds a COPY of
@@ -520,7 +552,8 @@ _ENGINES: "weakref.WeakKeyDictionary" = weakref.WeakKeyDictionary()
 
 def engine_for(model, device=None) -> DetrEngine:
     """The :class:`DetrEngine` behind ``model``: the engine itself, or one built (once) from a reference ``DETR``
-    ``nn.Module``'s ``state_dict()`` with ``nhead = model.transformer.nhead`` (DETR/models/detr.py:22, transformer.py:42)."""
+    ``nn.Module``'s ``state_dict()`` with ``nhead = model.transformer.nhead`` (DETR/models/detr.py:22, transformer.py:42)
+    and the DC5 dilation read from ``model.backbone[0].body.layer4[-1].conv2.dilation`` (DETR/models/backbone.py:88-90)."""
     if isinstance(model, DetrEngine):
         return model
     if not (hasattr(model, "state_dict") and callable(model.state_dict)):
@@ -531,6 +564,15 @@ def engine_for(model, device=None) -> DetrEngine:
             nhead = int(model.transformer.nhead)
         except (AttributeError, TypeError, ValueError):
             raise MmxError("a DETR module needs model.transformer.nhead (the reference Transformer sets it)") from None
-        eng = DetrEngine(model.state_dict(), nhead=nhead, device=device)
+        eng = DetrEngine(model.state_dict(), nhead=nhead, device=device, dilation=_module_dilation(model))
         _ENGINES[model] = eng
     return eng
+
+
+def _module_dilation(model) -> bool:
+    """True for a reference DETR module with a dilated (DC5) layer4; False when it has none or no backbone."""
+    try:
+        d = model.backbone[0].body.layer4[-1].conv2.dilation
+    except (AttributeError, IndexError, TypeError, KeyError):
+        return False
+    return int(d[0] if isinstance(d, (tuple, list)) else d) > 1
