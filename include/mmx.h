@@ -152,7 +152,8 @@ int mmx_bmm_add(const float* A, int lda, long long strideA, int transA, const fl
 #define MMX_ACT_NONE       0
 #define MMX_ACT_QUICKGELU  1   /* x*sigmoid(1.702x), CLIP/clip/model.py:162-164 */
 #define MMX_ACT_GELU       2   /* exact erf GELU (timm ViT, LXMERT) */
-#define MMX_ACT_RELU       3   /* DETR FFN, DETR/models/transformer.py:239 */
+#define MMX_ACT_RELU       3   /* DETR FFN, DETR/models/transformer.py:239; NaN propagates as in F.relu (relu(NaN) = NaN)
+                                  and the derivative passes the gradient where pre is NaN (threshold_backward) */
 #define MMX_ACT_TANH       4   /* LXMERT pooler, lxmert/lxmert/src/lxmert_lrp.py:868-884 */
 #define MMX_ACT_MUL        5   /* not an activation: the `pre` operand of a GEMM epilogue multiplies the product itself
                                   (C = (A W^T) (.) pre), the `x * (S W)` step of Linear.relprop, DETR/modules/layers.py:421-423 */

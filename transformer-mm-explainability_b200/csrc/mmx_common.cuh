@@ -137,7 +137,7 @@ __device__ __forceinline__ float act_fwd(float x, int act) {
   switch (act) {
     case MMX_ACT_QUICKGELU: return x / (1.f + expf(-1.702f * x));
     case MMX_ACT_GELU: return 0.5f * x * (1.f + erff(x * 0.70710678118654752f));
-    case MMX_ACT_RELU: return fmaxf(x, 0.f);
+    case MMX_ACT_RELU: return relu_nan(x);      // F.relu(NaN) = NaN: an overflow upstream stays visible
     case MMX_ACT_TANH: return tanhf(x);
     case MMX_ACT_SIGMOID: return 1.f / (1.f + expf(-x));
     default: return x;
@@ -154,7 +154,7 @@ __device__ __forceinline__ float act_bwd(float x, int act) {  // d act(x) / dx
       float pdf = 0.39894228040143268f * expf(-0.5f * x * x);
       return cdf + x * pdf;
     }
-    case MMX_ACT_RELU: return x > 0.f ? 1.f : 0.f;
+    case MMX_ACT_RELU: return x <= 0.f ? 0.f : 1.f;   // torch's threshold_backward: a NaN pre passes the gradient
     case MMX_ACT_TANH: { const float t = tanhf(x); return 1.f - t * t; }
     case MMX_ACT_MUL: return x;   // the epilogue multiplies by `pre` itself (Linear.relprop)
     case MMX_ACT_SIGMOID: { const float s = 1.f / (1.f + expf(-x)); return s * (1.f - s); }
