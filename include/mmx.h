@@ -284,6 +284,29 @@ int mmx_detr_position_sine(const uint8_t* mask, int B, int Hi, int Wi, int h, in
                            int ldpos, uint8_t* mask_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * DETR evaluation post-processing (the per-image body of DETR/engine.py:173-192, `--eval --masks`)
+ * ------------------------------------------------------------------------------------------------------- */
+
+/* PostProcess (DETR/models/detr.py:278-306) and the keep rule of MaskGenerator.get_panoptic (DETR/mask_generator.py:50-51)
+ * in one kernel, one warp per (image, query) row.  logits: pred_logits [B*Q, C1] (row stride ld, C1 = classes + 1 >= 2);
+ * prob = softmax(row); scores = max(prob[:C1-1]), labels = its index (int64; NaN wins, ties take the lower index, as
+ * torch's max(-1)); keep = scores > keep_threshold (bytes; false for NaN).  A row holding a NaN or inf gives score NaN.
+ * boxes: pred_boxes [B*Q, 4] (cx, cy, w, h); sizes: [B, 2] int64 (img_h, img_w), device memory;
+ * boxes_out = box_cxcywh_to_xyxy(boxes) * (img_w, img_h, img_w, img_h), the same bits as torch.  Every output may be
+ * NULL; boxes_out needs boxes and sizes. */
+int mmx_detr_postprocess(const float* logits, int ld, int B, int Q, int C1, float keep_threshold, float* scores, int64_t* labels,
+                         uint8_t* keep, const float* boxes, const int64_t* sizes, float* boxes_out, void* stream);
+/* PostProcessSegm (DETR/models/segmentation.py:218-242) for a batch in one launch: F.interpolate(pred_masks, (max_h, max_w),
+ * "bilinear", align_corners=False), sigmoid() > threshold, the crop [:img_h, :img_w] and F.interpolate(nearest) to
+ * (oh, ow), as bytes 0 / 1.  pred_masks: [B, Q, h, w] fp32 (any values; h > 1); sizes, orig_sizes: HOST int arrays [B][2]
+ * of (img_h, img_w) (target_sizes) and (oh, ow) (orig_target_sizes); (max_h, max_w) is the column max of sizes.
+ * out: device bytes, image i's [Q, oh_i, ow_i] masks at offset sum_{j<i} Q oh_j ow_j.  Only the bilinear values the
+ * nearest step reads are computed, with ATen's CUDA arithmetic, so the masks are the bits the reference's CUDA
+ * interpolate + CPU resize gives.  B <= 64. */
+int mmx_detr_segm_postprocess(const float* pred_masks, int B, int Q, int h, int w, const int* sizes, const int* orig_sizes,
+                              float threshold, uint8_t* out, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * CLIP engine: the north-star path (SURVEY.md §8a rows a1-a4), one call = interpret() for a batch.
  * ------------------------------------------------------------------------------------------------------- */
 

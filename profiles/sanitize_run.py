@@ -125,5 +125,14 @@ deng = mmx_b200.DetrEngine(dbo.init_state_dict(dbo.DETR_IMAGE, 3), nhead=dbo.DET
 for backend in (3, 1):
     l.mmx_set_gemm_backend(backend)
     deng(ims)
+# ---- DETR evaluation post-processing (detr_postprocess.cu): PostProcess with boxes, the keep-only launch, and the fused
+# PostProcessSegm on a padded two-image batch (16-byte and byte stores, crop) and on a same-size plane (the copy case)
+l.mmx_set_gemm_backend(3)
+pout = deng(ims)
+pout["pred_masks"] = torch.randn(2, dbo.DETR_IMAGE.queries, 5, 7, device="cuda")
+res = mmx_b200.PostProcess()(pout, torch.tensor([[70, 90], [64, 100]], device="cuda"))
+mmx_b200.detr_postprocess(pout["pred_logits"])
+mmx_b200.PostProcessSegm()(res, pout, torch.tensor([[61, 93], [33, 47]]), torch.tensor([[70, 90], [64, 100]]))
+mmx_b200.PostProcessSegm(0.85)(res[:1], {"pred_masks": pout["pred_masks"][:1]}, torch.tensor([[9, 21]]), torch.tensor([[5, 7]]))
 torch.cuda.synchronize()
 print("sanitize_run: all kernels executed")

@@ -18,7 +18,8 @@ from .synthetic import (clip_init_state_dict, clip_synthetic_inputs, DetrConfig,
                         detr_sine_position_embedding, detr_synthetic_inputs, LxmertConfig, LXMERT_BASE, LXMERT_TINY,
                         lxmert_init_state_dict, lxmert_synthetic_inputs)
 from .vit import ViTEngine, generate_relevance  # noqa: F401
-from .detr import DetrEngine, Generator, GeneratorAlbationNoAgg, MaskGenerator  # noqa: F401
+from .detr import (DetrEngine, Generator, GeneratorAlbationNoAgg, MaskGenerator, PostProcess, PostProcessSegm,  # noqa: F401
+                   detr_postprocess)
 from .backbone import DetrBackbone  # noqa: F401
 from .lxmert import LxmertEngine, GeneratorOurs, GeneratorBaselines, GeneratorOursAblationNoAggregation  # noqa: F401
 from .visualbert import VisualBertEngine, SelfAttentionGenerator  # noqa: F401

@@ -111,13 +111,13 @@ __global__ void __launch_bounds__(256) position_sine_kernel(const uint8_t* __res
   float* dim_t = sh + 2 * POS_PIX;
   uint8_t* nm = reinterpret_cast<uint8_t*>(dim_t + npf);
   const int b = blockIdx.x, n = h * w, p0 = blockIdx.y * POS_PIX, np_ = min(POS_PIX, n - p0);
-  // F.interpolate(m[None].float(), size=(h, w)) nearest (backbone.py:78): src = min(floor(dst * (float)in / out), in - 1)
+  // F.interpolate(m[None].float(), size=(h, w)) nearest (backbone.py:78)
   const float sy = (float)Hi / (float)h, sx = (float)Wi / (float)w;
   for (int p = threadIdx.x; p < n; p += blockDim.x) {
     const int y = p / w, x = p - y * w;
     uint8_t m = 0;
     if (mask) {
-      const int iy = min((int)floorf((float)y * sy), Hi - 1), ix = min((int)floorf((float)x * sx), Wi - 1);
+      const int iy = nearest_src(y, sy, Hi), ix = nearest_src(x, sx, Wi);
       m = mask[((long long)b * Hi + iy) * Wi + ix] != 0;
     }
     if (mask_out && p >= p0 && p < p0 + np_) mask_out[(long long)b * n + p] = m;

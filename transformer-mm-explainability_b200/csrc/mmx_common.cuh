@@ -133,6 +133,12 @@ __device__ __forceinline__ float warp_max(float v) {
 __device__ __forceinline__ float relu_nan(float x) { return x < 0.f ? 0.f : x; }
 __device__ __forceinline__ float min_nan(float m, float v) { return (v < m || v != v) ? v : m; }
 
+// Source index of torch's legacy "nearest" resampling (F.interpolate(mode="nearest"), the same rule on CPU and CUDA):
+// min(floor(dst * scale), in - 1) with scale = (float)in / (float)out.
+__device__ __forceinline__ int nearest_src(int dst, float scale, int in) {
+  return min((int)floorf((float)dst * scale), in - 1);
+}
+
 __device__ __forceinline__ float act_fwd(float x, int act) {
   switch (act) {
     case MMX_ACT_QUICKGELU: return x / (1.f + expf(-1.702f * x));

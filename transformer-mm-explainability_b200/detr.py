@@ -463,7 +463,9 @@ class MaskGenerator:
     """The relevance -> segmentation-mask step of DETR/mask_generator.py:39-125 (``get_panoptic``): one relevance map per
     kept query through the ``method`` switch (:93-113), then min-max / Otsu (:115-121).  The reference loops over the
     kept queries with one forward + backward and one CPU cv2 call each; here the queries of an image form ONE batch and
-    the masks come from one kernel launch.  The visualisation / COCO panoptic bookkeeping around it is out of scope.
+    the masks come from one kernel launch.  ``get_panoptic`` is the whole driver step (forward, keep rule, pred_masks);
+    ``PostProcess`` / ``PostProcessSegm`` below are the two post-processors the reference's ``evaluate`` runs after it.
+    The visualisation and the COCO evaluator are out of scope.
 
     The staged A / dA of every encoder layer grow with S^2 (about 2.4 GB per query at 2500 tokens, 6.8 GB at 4200), so the
     queries run in chunks: ``max_batch`` queries per chunk when given, else as many as the free device memory holds
@@ -513,12 +515,46 @@ class MaskGenerator:
         feats = self.model.features(img)
         if feats.B != 1:
             raise MmxError(f"get_masks segments one image, got a batch of {feats.B}")
-        h, w = feats.h, feats.w
+        return self._masks(feats, q, method, max_batch)
+
+    def _masks(self, feats: _Feats, q: torch.Tensor, method: str, max_batch: Optional[int]):
+        K, h, w = q.numel(), feats.h, feats.w
         lrp = method in ("ours_with_lrp", "transformer_att", "partial_lrp")
         n = int(max_batch) if max_batch is not None else self.chunk_size(h * w, lrp)
         cam = torch.cat([self._cams(feats.expand(len(qc)), qc, method) for qc in q.split(n)])
         masks, thr = rules.otsu_masks(cam)
         return masks.view(K, h, w), thr, cam
+
+    def get_panoptic(self, samples, targets, method: str, max_batch: Optional[int] = None):
+        """DETR/mask_generator.py:45-155: the segmentation driver's step 1 for one image (a [1,3,H,W] tensor, a one-image
+        list or a NestedTensor; ``targets`` is ignored, as in the reference).  One forward gives pred_logits / pred_boxes
+        and the keep rule ``softmax(pred_logits)[0, :, :-1].max(-1) > 0.5`` (mmx_detr_postprocess, on the device); the kept
+        queries go through ``get_masks`` on the same backbone features.  Returns {"pred_logits" [1,Q,C+1], "pred_boxes"
+        [1,Q,4], "pred_masks" [1,Q,h,w]} on the device, pred_masks -1 on the dropped queries and the {0, 255} Otsu mask on
+        the kept ones.  Prints "no segmentation" when at most one query is kept (:65-66).  An unknown ``method`` prints
+        and returns None before any work; the reference's two shape-probing forwards (:47, :80) are not needed."""
+        if method not in self.METHODS:
+            print("please provide a valid explainability method")            # mask_generator.py:111-113
+            return None
+        m = self.model
+        feats = m.features(samples)
+        if feats.B != 1:
+            raise MmxError(f"get_panoptic segments one image (the reference reads image 0 of --batch_size 1), got {feats.B}")
+        m._run(feats, None, backward=False)
+        if not m.bbox_embed:
+            raise MmxError("get_panoptic needs the box head (bbox_embed.*) in the state dict")
+        logits = m.pred_logits
+        boxes = m._boxes(m.saved["hs"].v)
+        keep = detr_postprocess(logits)["keep"][0]
+        q = keep.nonzero().flatten()                                           # one host sync, as keep.nonzero() there
+        K, Q, h, w = q.numel(), m.queries, feats.h, feats.w
+        if K <= 1:
+            print("no segmentation")
+        pred_masks = torch.full((1, Q, h, w), -1.0, device=m.device, dtype=torch.float32)
+        if K:
+            masks, _, _ = self._masks(feats, q, method, max_batch)
+            pred_masks.index_copy_(1, q, masks.view(1, K, h, w))
+        return {"pred_logits": logits, "pred_boxes": boxes, "pred_masks": pred_masks}
 
     def _cams(self, batch: _Feats, q: torch.Tensor, method: str) -> torch.Tensor:
         """the relevance maps [k, h*w] of the k queries ``q`` (one per sample of ``batch``) by ``method`` (:93-113)"""
@@ -543,6 +579,97 @@ class MaskGenerator:
         else:
             cam = self.gen.generate_partial_lrp(batch, q)
         return cam.reshape(q.numel(), -1)
+
+
+def detr_postprocess(pred_logits: torch.Tensor, pred_boxes: Optional[torch.Tensor] = None,
+                     target_sizes: Optional[torch.Tensor] = None, keep_threshold: float = 0.5) -> Dict[str, torch.Tensor]:
+    """One mmx_detr_postprocess launch over pred_logits [B,Q,C+1]: {"scores" [B,Q], "labels" [B,Q] int64, "keep" [B,Q] bool
+    (scores > keep_threshold)}, plus "boxes" [B,Q,4] (xyxy scaled by (w, h, w, h)) when pred_boxes and target_sizes [B,2]
+    (img_h, img_w) are given.  All on pred_logits' device."""
+    if pred_logits.dim() != 3:
+        raise MmxError(f"pred_logits is [B, Q, C+1], got {tuple(pred_logits.shape)}")
+    dev = pred_logits.device
+    x = _f32(pred_logits, dev)
+    B, Q, C1 = x.shape
+    scores = torch.empty(B, Q, device=dev, dtype=torch.float32)
+    labels = torch.empty(B, Q, device=dev, dtype=torch.int64)
+    keep = torch.empty(B, Q, device=dev, dtype=torch.uint8)
+    out = {"scores": scores, "labels": labels}
+    bx = sz = bo = None
+    if pred_boxes is not None and target_sizes is not None:
+        if tuple(pred_boxes.shape) != (B, Q, 4) or tuple(target_sizes.shape) != (B, 2):
+            raise MmxError(f"pred_boxes [B,Q,4] and target_sizes [B,2] for pred_logits {tuple(x.shape)}, got "
+                           f"{tuple(pred_boxes.shape)} and {tuple(target_sizes.shape)}")
+        bx = _f32(pred_boxes, dev)
+        sz = target_sizes.to(device=dev, dtype=torch.int64).contiguous()
+        bo = torch.empty(B, Q, 4, device=dev, dtype=torch.float32)
+    with torch.cuda.device(dev):
+        check(lib().mmx_detr_postprocess(ptr(x), C1, B, Q, C1, float(keep_threshold), ptr(scores), ptr(labels), ptr(keep),
+                                         ptr(bx), ptr(sz), ptr(bo), current_stream()))
+    out["keep"] = keep.bool()
+    if bo is not None:
+        out["boxes"] = bo
+    return out
+
+
+class PostProcess:
+    """``PostProcess`` (DETR/models/detr.py:278-306): softmax, score / label per query (max over the classes, the
+    no-object column excluded) and the boxes as xyxy in pixels of ``target_sizes`` [B,2] (img_h, img_w), in one
+    kernel.  Returns the reference's list of {"scores", "labels", "boxes"} per image, on the device."""
+
+    @torch.no_grad()
+    def forward(self, outputs, target_sizes):
+        out_logits, out_bbox = outputs["pred_logits"], outputs["pred_boxes"]
+        assert len(out_logits) == len(target_sizes)
+        assert target_sizes.shape[1] == 2
+        r = detr_postprocess(out_logits, out_bbox, target_sizes)
+        return [{"scores": s, "labels": l, "boxes": b} for s, l, b in zip(r["scores"], r["labels"], r["boxes"])]
+
+    __call__ = forward
+
+
+class PostProcessSegm:
+    """``PostProcessSegm`` (DETR/models/segmentation.py:218-242): adds "masks" - uint8 [Q,1,oh,ow] on the CPU, 0 / 1 -
+    to each result.  The bilinear resize to the batch's max size, ``sigmoid() > threshold``, the crop to each image's
+    ``max_target_sizes`` row and the nearest resize to its ``orig_target_sizes`` row run as ONE kernel launch
+    (mmx_detr_segm_postprocess), and only the final uint8 masks cross to the host, in one copy.  The reference instead
+    materialises the fp32 bilinear masks at the padded size, copies them to the host as bool and resizes them there."""
+
+    def __init__(self, threshold: float = 0.5):
+        self.threshold = threshold
+
+    @torch.no_grad()
+    def forward(self, results, outputs, orig_target_sizes, max_target_sizes):
+        assert len(orig_target_sizes) == len(max_target_sizes)
+        masks = outputs["pred_masks"]
+        if masks.dim() == 5 and masks.shape[2] == 1:                       # the .squeeze(2) of :227
+            masks = masks[:, :, 0]
+        if masks.dim() != 4 or masks.shape[2] == 1:
+            raise MmxError(f"pred_masks is [B, Q, h, w] with h > 1, got {tuple(outputs['pred_masks'].shape)}")
+        B, Q, h, w = masks.shape
+        sizes = [tuple(int(v) for v in t) for t in max_target_sizes.tolist()]
+        orig = [tuple(int(v) for v in t) for t in orig_target_sizes.tolist()]
+        if len(sizes) != B or len(results) != B:
+            raise MmxError(f"{B} images of pred_masks, {len(sizes)} target sizes and {len(results)} results")
+        if min(min(s) for s in sizes + orig) <= 0:
+            raise MmxError(f"image sizes must be positive, got {sizes} and {orig}")
+        dev = masks.device
+        x = _f32(masks, dev)
+        n = [Q * oh * ow for oh, ow in orig]
+        buf = torch.empty(sum(n), device=dev, dtype=torch.uint8)
+        flat_sizes = (C.c_int * (2 * B))(*[v for s in sizes for v in s])
+        flat_orig = (C.c_int * (2 * B))(*[v for s in orig for v in s])
+        with torch.cuda.device(dev):
+            check(lib().mmx_detr_segm_postprocess(ptr(x), B, Q, h, w, flat_sizes, flat_orig, float(self.threshold),
+                                                  ptr(buf), current_stream()))
+            host = torch.empty(buf.numel(), dtype=torch.uint8, pin_memory=True)
+            host.copy_(buf, non_blocking=True)
+            torch.cuda.current_stream().synchronize()
+        for r, part, (oh, ow) in zip(results, host.split(n), orig):
+            r["masks"] = part.view(Q, 1, oh, ow)
+        return results
+
+    __call__ = forward
 
 
 # Engines built from reference ``DETR`` modules, keyed by the module object (dropped with it).  The engine holds a COPY of
