@@ -71,7 +71,8 @@ int mmx_avg_heads(const float* A, const float* dA, float* Abar, int B, int H, in
 
 /* attn-GradCAM baseline:  out[b,t,s] = relu( (1/H) sum_h A[b,h,t,s] * mean_{t',s'} dA[b,h,t',s'] ).
  * Replaces gradcam() (DETR/modules/ExplanationGenerator.py:275-280; lxmert/lxmert/src/ExplanationGenerator.py:542-547).
- * gbar: device scratch of B*H floats. */
+ * gbar: device scratch of B*H floats; each plane mean is summed in double, so it is the fp32 rounding of the exact mean
+ * even when a signed gradient nearly cancels over a long plane (T = S = 2500). */
 int mmx_attn_gradcam(const float* A, const float* dA, float* out, float* gbar, int B, int H, int T, int S, int ld_in,
                      int ld_out, void* stream);
 
@@ -124,17 +125,22 @@ int mmx_rollout(const float* mats, int L, int B, int S, int start_layer, int nor
 /* Min-max normalisation of B contiguous maps of n floats: Y = (X - min X) / (max X - min X) per map (in place allowed).
  * Replaces the `(cam - cam.min()) / (cam.max() - cam.min())` step of the attn-GradCAM / partial-LRP baselines
  * (VisualBERT/mmf/models/transformers/backends/ExplanationGenerator.py:122,203) and of the DETR mask generator
- * (DETR/mask_generator.py:115-121).  A constant map yields NaN, as in the reference. */
+ * (DETR/mask_generator.py:115-121).  A constant map yields NaN, as in the reference.  min and max propagate NaN as
+ * torch's cam.min() / cam.max() do: a map holding a NaN yields NaN everywhere. */
 int mmx_minmax_normalize(const float* X, float* Y, int B, long long n, void* stream);
 
 /* Otsu masks for B relevance maps of n floats (the step right after the path in the DETR segmentation driver):
  * masks[b] = 255 where uint8((cam - min) / (max - min) * 255) > otsu_threshold else 0, thresholds[b] (optional) = the
  * threshold.  Replaces DETR/mask_generator.py:115-121 (`cv2.threshold(..., THRESH_BINARY + THRESH_OTSU)` on the CPU with
- * a device->host->device round trip per query); bit-identical to OpenCV's getThreshVal_Otsu_8u. */
+ * a device->host->device round trip per query); bit-identical to OpenCV's getThreshVal_Otsu_8u.  A map holding a NaN
+ * (or a constant map) normalises to NaN everywhere, which the uint8 cast turns into 0 as numpy does on x86: threshold 0,
+ * mask all 0. */
 int mmx_otsu_masks(const float* cams, float* masks, int* thresholds, int B, int n, void* stream);
 
 /* Top-k selection for the perturbation drivers: for each of B rows of n scores, keep[b][i] = 1 for the k[b] highest
  * scores (ties: lower index first), pos[b][i] = rank of i among the kept elements in index order, -1 when dropped.
+ * NaN ranks above every number, as in torch.topk (among NaNs the lower index first); exactly clamp(k[b], 0, n) elements
+ * are kept.  n <= 4096.
  * Replaces `cam.topk(k)` + host-side `sorted(...)` + gather (lxmert/lxmert/perturbation.py:110-117,160-178). */
 int mmx_topk_select(const float* scores, const int* k, int* keep, int* pos, int B, int n, void* stream);
 

@@ -10,21 +10,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 INDIRECT = {
     "mmx_version": "test_capi.py (CPU) and build()",
     "mmx_last_error": "library state: its text is the message of every MmxError the GPU tests raise",
-    "mmx_launch_count": "library state: read by bench.py and smoke() for the launch count",
     "mmx_profile_gemm": "bench.py's GEMM roofline line: timing only, no result to compare",
     "mmx_profile_gemm_report": "bench.py's GEMM roofline line: timing only, no result to compare",
     "mmx_gemm_trace": "profiling aid (profiles/attn_trace.py); it only sets a pointer",
     "mmx_memcpy_d2d": "through ClipEngine.tap, test_clip_gpu.py",
-    "mmx_avg_heads": "through rules.avg_heads_batched, test_rules_gpu.py",
-    "mmx_attn_gradcam": "through the attn-GradCAM baseline (GeneratorBaselines), test_detr_lxmert_gpu.py",
-    "mmx_self_update": "through the rule-6/7 updates of every Generator, test_detr_lxmert_gpu.py",
-    "mmx_handle_residual": "through rules.apply_mm_attention_rules_*, test_rules_gpu.py",
-    "mmx_mm_update_workspace": "through rules.apply_mm_attention_rules_*, test_rules_gpu.py",
-    "mmx_mm_update": "through rules.apply_mm_attention_rules_*, test_rules_gpu.py",
-    "mmx_rollout": "through rules.compute_rollout_attention, test_rules_gpu.py",
-    "mmx_minmax_normalize": "through mmx_b200.minmax_normalize, test_detr_lxmert_gpu.py",
-    "mmx_otsu_masks": "through mmx_b200.otsu_masks, test_detr_lxmert_gpu.py",
-    "mmx_topk_select": "through mmx_b200.topk_select, test_perturbation_gpu.py",
     "mmx_linear": "mmx_linear_packed with packed = NULL, test_primitives_gpu.py",
     "mmx_linear_dgrad": "mmx_linear_dgrad_packed with packed = NULL, test_primitives_gpu.py",
     "mmx_clip_create": "ClipEngine object, test_clip_gpu.py",
@@ -35,17 +24,6 @@ INDIRECT = {
     "mmx_clip_interpret_host": "ClipEngine object, test_clip_gpu.py",
     "mmx_clip_set_serial": "ClipEngine object, test_clip_gpu.py",
     "mmx_clip_tap": "ClipEngine object, test_clip_gpu.py",
-    "mmx_lrp_split": "through mmx_b200.lrp (the use_lrp=True sweeps), test_lrp_gpu.py",
-    "mmx_lrp_safe_divide": "through mmx_b200.lrp (the use_lrp=True sweeps), test_lrp_gpu.py",
-    "mmx_lrp_partials_len": "through mmx_b200.lrp (the use_lrp=True sweeps), test_lrp_gpu.py",
-    "mmx_lrp_sums": "through mmx_b200.lrp (the use_lrp=True sweeps), test_lrp_gpu.py",
-    "mmx_lrp_renorm": "through mmx_b200.lrp (the use_lrp=True sweeps), test_lrp_gpu.py",
-    "mmx_lrp_add": "through mmx_b200.lrp (the use_lrp=True sweeps), test_lrp_gpu.py",
-    "mmx_lrp_clone": "through mmx_b200.lrp (the use_lrp=True sweeps), test_lrp_gpu.py",
-    "mmx_lrp_zero_value_fix": "through mmx_b200.lrp (the use_lrp=True sweeps), test_lrp_gpu.py",
-    "mmx_lrp_attn_pv": "through mmx_b200.lrp (the use_lrp=True sweeps), test_lrp_gpu.py",
-    "mmx_lrp_attn_qk": "through mmx_b200.lrp (the use_lrp=True sweeps), test_lrp_gpu.py",
-    "mmx_lrp_attn_scores": "through SelfAttentionGenerator.generate_transformer_att (VisualBERT), test_lrp_gpu.py",
 }
 
 

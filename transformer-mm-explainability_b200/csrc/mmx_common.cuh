@@ -128,10 +128,11 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
-// clamp(min=0) and min() with torch's NaN semantics (NaN propagates; fmaxf / fminf would drop it): a numerical blow-up
+// clamp(min=0), min() and max() with torch's NaN semantics (NaN propagates; fmaxf / fminf would drop it): a numerical blow-up
 // upstream must reach the caller (and trip the reference's `assert diag(R - I).min() >= 0`) instead of being masked.
 __device__ __forceinline__ float relu_nan(float x) { return x < 0.f ? 0.f : x; }
 __device__ __forceinline__ float min_nan(float m, float v) { return (v < m || v != v) ? v : m; }
+__device__ __forceinline__ float max_nan(float m, float v) { return (v > m || v != v) ? v : m; }
 
 // Source index of torch's legacy "nearest" resampling (F.interpolate(mode="nearest"), the same rule on CPU and CUDA):
 // min(floor(dst * scale), in - 1) with scale = (float)in / (float)out.

@@ -54,20 +54,22 @@ __global__ void __launch_bounds__(256) avg_heads_vec4_kernel(const float* __rest
 }
 
 // attn-GradCAM baseline (DETR/modules/ExplanationGenerator.py:275-280): gbar[b,h] = mean_{t,s} dA[b,h,t,s], then
-// out[b,t,s] = relu((1/H) sum_h A[b,h,t,s] * gbar[b,h]).
+// out[b,t,s] = relu((1/H) sum_h A[b,h,t,s] * gbar[b,h]).  The plane sum runs in double: at DETR's long planes
+// (T = S = 2500) each thread adds ~24k terms, and a signed gradient's mean can nearly cancel.
 __global__ void __launch_bounds__(256) plane_mean_kernel(const float* __restrict__ G, float* __restrict__ gbar, int T, int S,
                                                          int ld) {
-  __shared__ float red[8];
+  __shared__ double red[8];
   const float* g = G + (long long)blockIdx.x * T * ld;
-  float acc = 0.f;
-  for (int e = threadIdx.x; e < T * S; e += blockDim.x) acc += g[(long long)(e / S) * ld + e % S];
-  acc = warp_sum(acc);
+  double acc = 0.0;
+  for (int e = threadIdx.x; e < T * S; e += blockDim.x) acc += (double)g[(long long)(e / S) * ld + e % S];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
   __syncthreads();
   if (threadIdx.x == 0) {
-    float t = 0.f;
+    double t = 0.0;
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += red[w];
-    gbar[blockIdx.x] = t / (float)((long long)T * S);
+    gbar[blockIdx.x] = (float)(t / ((double)T * S));
   }
 }
 __global__ void __launch_bounds__(256) gradcam_kernel(const float* __restrict__ A, const float* __restrict__ gbar,
@@ -344,20 +346,30 @@ int copy2d(const float* src, int lds, float* dst, int ldd, long long rows, int c
   return 0;
 }
 
-// y = (x - min(x)) / (max(x) - min(x)) over each of B contiguous maps of n floats (one CTA per map).  A constant map
-// gives 0/0 = NaN exactly as the reference expression does.
-__global__ void __launch_bounds__(256) minmax_normalize_kernel(const float* __restrict__ X, float* __restrict__ Y, long long n) {
-  const float* x = X + (long long)blockIdx.x * n;
-  float* y = Y + (long long)blockIdx.x * n;
-  float mn = INFINITY, mx = -INFINITY;
-  for (long long i = threadIdx.x; i < n; i += blockDim.x) { const float v = x[i]; mn = fminf(mn, v); mx = fmaxf(mx, v); }
+// min and max of one map over a 256-thread CTA, as torch's cam.min() / cam.max(): one NaN makes both NaN (fminf / fmaxf
+// would skip it).  Every thread gets the result.
+__device__ __forceinline__ void block_minmax_nan(float& mn, float& mx) {
   __shared__ float smn[8], smx[8];
-  mn = -warp_max(-mn); mx = warp_max(mx);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    mn = min_nan(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+    mx = max_nan(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  }
   if ((threadIdx.x & 31) == 0) { smn[threadIdx.x >> 5] = mn; smx[threadIdx.x >> 5] = mx; }
   __syncthreads();
   mn = smn[0]; mx = smx[0];
 #pragma unroll
-  for (int w = 1; w < 8; ++w) { mn = fminf(mn, smn[w]); mx = fmaxf(mx, smx[w]); }
+  for (int w = 1; w < 8; ++w) { mn = min_nan(mn, smn[w]); mx = max_nan(mx, smx[w]); }
+}
+
+// y = (x - min(x)) / (max(x) - min(x)) over each of B contiguous maps of n floats (one CTA per map).  A constant map
+// gives 0/0 = NaN and a map holding a NaN gives NaN everywhere, exactly as the reference expression does.
+__global__ void __launch_bounds__(256) minmax_normalize_kernel(const float* __restrict__ X, float* __restrict__ Y, long long n) {
+  const float* x = X + (long long)blockIdx.x * n;
+  float* y = Y + (long long)blockIdx.x * n;
+  float mn = INFINITY, mx = -INFINITY;
+  for (long long i = threadIdx.x; i < n; i += blockDim.x) { const float v = x[i]; mn = min_nan(mn, v); mx = max_nan(mx, v); }
+  block_minmax_nan(mn, mx);
   const float d = mx - mn;
   for (long long i = threadIdx.x; i < n; i += blockDim.x) y[i] = (x[i] - mn) / d;
 }
@@ -369,23 +381,17 @@ __global__ void __launch_bounds__(256) otsu_mask_kernel(const float* __restrict_
                                                        int* __restrict__ thresholds, int n) {
   const float* x = X + (long long)blockIdx.x * n;
   float* m = M + (long long)blockIdx.x * n;
-  __shared__ float smn[8], smx[8];
   __shared__ int hist[256];
   __shared__ int s_thr;
   float mn = INFINITY, mx = -INFINITY;
-  for (int i = threadIdx.x; i < n; i += blockDim.x) { const float v = x[i]; mn = fminf(mn, v); mx = fmaxf(mx, v); }
-  mn = -warp_max(-mn); mx = warp_max(mx);
-  if ((threadIdx.x & 31) == 0) { smn[threadIdx.x >> 5] = mn; smx[threadIdx.x >> 5] = mx; }
+  for (int i = threadIdx.x; i < n; i += blockDim.x) { const float v = x[i]; mn = min_nan(mn, v); mx = max_nan(mx, v); }
   hist[threadIdx.x] = 0;
-  __syncthreads();
-  mn = smn[0]; mx = smx[0];
-#pragma unroll
-  for (int w = 1; w < 8; ++w) { mn = fminf(mn, smn[w]); mx = fmaxf(mx, smx[w]); }
+  block_minmax_nan(mn, mx);                                  // its barrier also orders the histogram clear
   const float d = mx - mn;
   auto quant = [&](float v) -> int {                       // ((v - min) / (max - min)) * 255 in fp32, then astype(uint8)
     const float q = __fmul_rn(__fdiv_rn(__fsub_rn(v, mn), d), 255.f);
-    return q >= 0.f ? (int)q & 255 : 0;                      // NaN (constant map) -> 0, as numpy's cast gives on x86
-  };
+    return q >= 0.f ? (int)q & 255 : 0;                      // NaN (constant map, or a NaN anywhere in it) -> 0, as numpy's
+  };                                                         // cast gives on x86: every pixel lands in bin 0, mask all 0
   for (int i = threadIdx.x; i < n; i += blockDim.x) atomicAdd(&hist[quant(x[i])], 1);
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -417,9 +423,10 @@ __global__ void __launch_bounds__(256) otsu_mask_kernel(const float* __restrict_
 }
 
 // Top-k selection by rank for the perturbation drivers (lxmert/lxmert/perturbation.py:110-113,160-172: `cam.topk(k)` then
-// gather): keep[i] = 1 if fewer than k elements beat element i (greater score, or equal score and lower index),
-// pos[i] = number of kept elements before i in INDEX order (the compacted position after the reference's `sorted`), or -1.
-// One CTA per row; n <= 4096.
+// gather): keep[i] = 1 if fewer than k elements beat element i (greater score, or equal score and lower index; a NaN
+// beats every number, as torch.topk ranks it, and NaNs among themselves follow the index rule), pos[i] = number of kept
+// elements before i in INDEX order (the compacted position after the reference's `sorted`), or -1.  The ranks are a
+// permutation of 0..n-1, so exactly clamp(k, 0, n) elements are kept.  One CTA per row; n <= 4096.
 __global__ void __launch_bounds__(256) topk_select_kernel(const float* __restrict__ scores, int n, const int* __restrict__ k,
                                                          int* __restrict__ keep, int* __restrict__ pos) {
   extern __shared__ float sh[];
@@ -431,8 +438,12 @@ __global__ void __launch_bounds__(256) topk_select_kernel(const float* __restric
   __syncthreads();
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     const float v = sv[i];
+    const bool v_nan = v != v;
     int rank = 0;
-    for (int j = 0; j < n; ++j) rank += (sv[j] > v) || (sv[j] == v && j < i);
+    for (int j = 0; j < n; ++j) {
+      const float u = sv[j];
+      rank += (u != u) ? (!v_nan || j < i) : (!v_nan && (u > v || (u == v && j < i)));
+    }
     sk[i] = rank < kk;
   }
   __syncthreads();
