@@ -410,6 +410,48 @@ int mmx_lrp_attn_qk(const float* cam1, int ldA, const float* Q, int ldq, const f
 int mmx_lrp_attn_scores(const float* Q, int ldq, const float* K, int ldk, const float* key_bias, float zscale, float* scores,
                         float* mask, int ldA, int B, int H, int T, int S, int hd, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * DETR's evaluation losses (DETR/engine.py:174 `criterion(outputs, targets)`): HungarianMatcher (DETR/models/matcher.py)
+ * and SetCriterion (DETR/models/detr.py:103-275, DETR/models/segmentation.py:172-215), for the last decoder layer and the
+ * auxiliary ones (DETR.forward's aux_outputs, detr.py:70-77, 95-100).  Shared layout: L layers (layer 0 the model's final
+ * output, 1 .. L-1 aux_outputs 0 .. L-2; logits / boxes: host arrays of L device pointers to [B,Q,C1] and [B,Q,4]
+ * contiguous fp32), B <= 64 images, Q queries.  The targets of all images are concatenated: tgt_ids [T] int64, tgt_boxes
+ * [T,4] cxcywh fp32; tgt_offsets is a HOST array [B+1] (0, ..., T), image b owning targets off[b] .. off[b+1].
+ * cost: the [Q, T_b] block of (layer l, image b) at l*Q*T + Q*off[b], row-major (the blocks kept after C.split(sizes),
+ * matcher.py:80-81).  indices [L,2,T] int64: indices[l][0][off[b]+k] the query (ascending) and indices[l][1][off[b]+k]
+ * the target of pair k < min(Q, T_b); unused slots -1.  Nothing here waits for the device.
+ * ------------------------------------------------------------------------------------------------------- */
+/* C = w_bbox cdist_L1 + w_class (-softmax(logits)[:, tgt_ids]) + w_giou (-GIoU) (matcher.py:60-77): the softmax in
+ * mmx_detr_postprocess's order, GIoU in box_ops' order (DETR/util/box_ops.py:22-68).  status [L] int (device, zeroed
+ * here): bit 1 when a predicted box of layer l - or, in status[0], a target box - fails generalized_box_iou's
+ * `x1 >= x0 and y1 >= y0` assert (box_ops.py:51-52, NaN included); bit 2 in status[0] for a label outside [0, C1). */
+int mmx_detr_match_cost(const float* const* logits, const float* const* boxes, int L, int B, int Q, int C1,
+                        const int64_t* tgt_ids, const float* tgt_boxes, const int* tgt_offsets, float w_class, float w_bbox,
+                        float w_giou, float* cost, int* status, void* stream);
+/* scipy.optimize.linear_sum_assignment (matcher.py:81) of every (layer, image) cost block in one launch, one CTA each: the
+ * shortest-augmenting-path algorithm scipy implements (Crouse 2016) restated in double, with its transpose of a tall
+ * matrix, row order, column scan order, tie rule and dual updates, so ties resolve as scipy resolves them.  Q and every
+ * T_b at most 1024.  status [L*B] int (device, zeroed here): 1 = a NaN or -inf entry ("matrix contains invalid numeric
+ * entries"), 2 = no finite complete assignment ("cost matrix is infeasible"). */
+int mmx_detr_match_lsa(const float* cost, int L, int B, int Q, const int* tgt_offsets, int64_t* indices, int* status,
+                       void* stream);
+/* The box and label losses of every layer (detr.py:124-188): out [L,5] = loss_ce (F.cross_entropy with empty_weight [C1]
+ * over the B*Q rows, unmatched rows taking class C1-1), class_error (100 - top-1 accuracy of the matched rows, 100 when
+ * none; util/misc.py:432-447; the top-1 is CUDA topk(1)'s: the lowest index among equal maxima, NaN above numbers), loss_bbox (sum |src - tgt| / num_boxes), loss_giou (sum (1 - GIoU) / num_boxes),
+ * cardinality_error (mean over images of |#(argmax != C1-1) - T_b|).  num_boxes: one device float (detr.py:248-252).
+ * Sums are doubles reduced in a fixed order. */
+int mmx_detr_set_losses(const float* const* logits, const float* const* boxes, int L, int B, int Q, int C1,
+                        const int64_t* tgt_ids, const float* tgt_boxes, const int* tgt_offsets, const int64_t* indices,
+                        const float* empty_weight, const float* num_boxes, float* out, void* stream);
+/* loss_masks (DETR/models/detr.py:184-211; focal and dice, segmentation.py:172-215) of one layer: each matched query's
+ * pred_masks [B,Q,h,w] plane upsampled bilinearly (align_corners=False, ATen's arithmetic) to the padded target size
+ * (max H_b, max W_b), the target read in place from tgt_masks[b] ([T_b, H_b, W_b], tgt_hw host [2B]; uint8 / bool for mask_dtype 0, fp32 for 1) and zero beyond its
+ * image; out [2] = sigmoid focal loss (alpha 0.25, gamma 2, mean over pixels) and dice loss, each summed over the masks and
+ * divided by num_boxes; both 0 when no image has a target.  indices: the [2,T] block of the layer.  Per-mask partial sums are doubles in a fixed order. */
+int mmx_detr_mask_losses(const float* pred_masks, int B, int Q, int h, int w, const void* const* tgt_masks, const int* tgt_hw,
+                         int mask_dtype, const int* tgt_offsets, const int64_t* indices, const float* num_boxes, float* out,
+                         void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -21,6 +21,7 @@ from .vit import ViTEngine, generate_relevance  # noqa: F401
 from .detr import (DetrEngine, Generator, GeneratorAlbationNoAgg, MaskGenerator, PostProcess, PostProcessSegm,  # noqa: F401
                    detr_postprocess)
 from .backbone import DetrBackbone  # noqa: F401
+from .criterion import HungarianMatcher, SetCriterion  # noqa: F401
 from .lxmert import LxmertEngine, GeneratorOurs, GeneratorBaselines, GeneratorOursAblationNoAggregation  # noqa: F401
 from .visualbert import VisualBertEngine, SelfAttentionGenerator  # noqa: F401
 from .perturbation import LxmertPerturbation, VisualBertPerturbation, PERT_STEPS, topk_select  # noqa: F401

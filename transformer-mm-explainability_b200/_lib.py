@@ -113,6 +113,17 @@ _SIGS = {
                                        C.c_void_p, c_float_p, C.c_void_p, c_float_p, C.c_void_p]),
     "mmx_detr_segm_postprocess": (C.c_int, [c_float_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int),
                                             C.POINTER(C.c_int), C.c_float, C.c_void_p, C.c_void_p]),
+    "mmx_detr_match_cost": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int,
+                                      C.c_void_p, c_float_p, C.POINTER(C.c_int), C.c_float, C.c_float, C.c_float, c_float_p,
+                                      C.c_void_p, C.c_void_p]),
+    "mmx_detr_match_lsa": (C.c_int, [c_float_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.c_void_p, C.c_void_p,
+                                     C.c_void_p]),
+    "mmx_detr_set_losses": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int,
+                                      C.c_void_p, c_float_p, C.POINTER(C.c_int), C.c_void_p, c_float_p, c_float_p, c_float_p,
+                                      C.c_void_p]),
+    "mmx_detr_mask_losses": (C.c_int, [c_float_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p),
+                                       C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int), C.c_void_p, c_float_p, c_float_p,
+                                       C.c_void_p]),
     "mmx_clip_create": (C.c_int, [C.POINTER(ClipConfigC), C.c_int, C.POINTER(C.c_void_p)]),
     "mmx_clip_destroy": (None, [C.c_void_p]),
     "mmx_clip_load_tensor": (C.c_int, [C.c_void_p, C.c_char_p, c_float_p, C.c_size_t]),

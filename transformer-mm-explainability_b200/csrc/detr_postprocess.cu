@@ -20,15 +20,6 @@ constexpr int PP_WARPS = 8;            // rows of pred_logits per CTA of the pos
 constexpr int SEGM_ROWS = 16;          // output rows per CTA of the segmentation kernel
 constexpr int SEGM_MAX_IMAGES = 64;    // images per call (the per-image geometry is a kernel parameter)
 
-// torch's max(-1) order (GreaterOrNan): a NaN beats any number, equal values keep the lower index.
-__device__ __forceinline__ bool better(float a, int ia, float b, int ib) {
-  if (ib < 0) return ia >= 0;
-  if (ia < 0) return false;
-  if (a != a) return b != b ? ia < ib : true;
-  if (b != b) return false;
-  return a > b || (a == b && ia < ib);
-}
-
 __global__ void __launch_bounds__(PP_WARPS * 32) detr_postprocess_kernel(
     const float* __restrict__ logits, int ld, int rows, int Q, int C1, float keep_thr, float* __restrict__ scores,
     long long* __restrict__ labels, uint8_t* __restrict__ keep, const float* __restrict__ boxes,
@@ -37,24 +28,20 @@ __global__ void __launch_bounds__(PP_WARPS * 32) detr_postprocess_kernel(
   if (r >= rows) return;
   const float* x = logits + (long long)r * ld;
   // softmax over the C + 1 columns, as torch's warp softmax orders it
-  float m = -INFINITY;
-  for (int c = lane; c < C1; c += 32) { const float v = x[c]; m = m > v ? m : v; }
-  m = warp_max(m);
-  float s = 0.f;
-  for (int c = lane; c < C1; c += 32) s += expf(x[c] - m);
-  s = warp_sum(s);
+  float m, s;
+  warp_softmax_stats(x, C1, lane, m, s);
   // max / argmax of prob[:C]; a NaN or inf logit makes every prob NaN (the sum is NaN), as in torch
   float best = 0.f;
   int bi = -1;
   for (int c = lane; c < C1 - 1; c += 32) {
     const float p = expf(x[c] - m) / s;
-    if (better(p, c, best, bi)) { best = p; bi = c; }
+    if (argmax_better(p, c, best, bi)) { best = p; bi = c; }
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     const float ob = __shfl_xor_sync(0xffffffffu, best, o);
     const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (better(ob, oi, best, bi)) { best = ob; bi = oi; }
+    if (argmax_better(ob, oi, best, bi)) { best = ob; bi = oi; }
   }
   if (lane == 0) {
     if (scores) scores[r] = best;
@@ -80,17 +67,6 @@ struct SegmImage {
 struct SegmBatch {
   SegmImage im[SEGM_MAX_IMAGES];
 };
-
-// ATen's area_pixel_compute_source_index (align_corners=False, linear): max(scale (dst + 0.5) - 0.5, 0), then the two taps
-// and the weight of the second (UpSample.cuh; upsample_bilinear2d_out_frame).  The expression is written as ATen writes it,
-// so nvcc contracts it the same way (one fma).
-__device__ __forceinline__ void linear_taps(int dst, float scale, int in, int& i0, int& i1, float& l1) {
-  const float src = scale * ((float)dst + 0.5f) - 0.5f;
-  const float r = src < 0.f ? 0.f : src;
-  i0 = (int)r;
-  i1 = i0 + (i0 < in - 1 ? 1 : 0);
-  l1 = r - (float)i0;
-}
 
 // Grid (ceil(max oh / SEGM_ROWS), Q, B).  Shared memory: the [h, w] plane, then per output column the packed taps
 // (x0 | x1 << 16) and the weight of x1, then the same per output row of the CTA.

@@ -128,16 +128,49 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
+// Row max and sum of exp(x - max) of a softmax over the n columns of x, in the order torch's warp softmax uses for rows of
+// up to 1024 columns: per-lane partials over columns lane, lane + 32, ..., then a butterfly.  Every lane of the warp gets
+// both; prob[c] = expf(x[c] - m) / s.
+__device__ __forceinline__ void warp_softmax_stats(const float* x, int n, int lane, float& m, float& s) {
+  m = -INFINITY;
+  for (int c = lane; c < n; c += 32) { const float v = x[c]; m = m > v ? m : v; }
+  m = warp_max(m);
+  s = 0.f;
+  for (int c = lane; c < n; c += 32) s += expf(x[c] - m);
+  s = warp_sum(s);
+}
+
 // clamp(min=0), min() and max() with torch's NaN semantics (NaN propagates; fmaxf / fminf would drop it): a numerical blow-up
 // upstream must reach the caller (and trip the reference's `assert diag(R - I).min() >= 0`) instead of being masked.
 __device__ __forceinline__ float relu_nan(float x) { return x < 0.f ? 0.f : x; }
 __device__ __forceinline__ float min_nan(float m, float v) { return (v < m || v != v) ? v : m; }
 __device__ __forceinline__ float max_nan(float m, float v) { return (v > m || v != v) ? v : m; }
 
+// torch's max(-1) / argmax order (GreaterOrNan): a NaN beats any number, equal values keep the lower index; index -1 is
+// "no candidate yet".
+__device__ __forceinline__ bool argmax_better(float a, int ia, float b, int ib) {
+  if (ib < 0) return ia >= 0;
+  if (ia < 0) return false;
+  if (a != a) return b != b ? ia < ib : true;
+  if (b != b) return false;
+  return a > b || (a == b && ia < ib);
+}
+
 // Source index of torch's legacy "nearest" resampling (F.interpolate(mode="nearest"), the same rule on CPU and CUDA):
 // min(floor(dst * scale), in - 1) with scale = (float)in / (float)out.
 __device__ __forceinline__ int nearest_src(int dst, float scale, int in) {
   return min((int)floorf((float)dst * scale), in - 1);
+}
+
+// ATen's area_pixel_compute_source_index (align_corners=False, linear): max(scale (dst + 0.5) - 0.5, 0), then the two taps
+// and the weight of the second (UpSample.cuh; upsample_bilinear2d_out_frame).  The expression is written as ATen writes it,
+// so nvcc contracts it the same way (one fma).
+__device__ __forceinline__ void linear_taps(int dst, float scale, int in, int& i0, int& i1, float& l1) {
+  const float src = scale * ((float)dst + 0.5f) - 0.5f;
+  const float r = src < 0.f ? 0.f : src;
+  i0 = (int)r;
+  i1 = i0 + (i0 < in - 1 ? 1 : 0);
+  l1 = r - (float)i0;
 }
 
 __device__ __forceinline__ float act_fwd(float x, int act) {

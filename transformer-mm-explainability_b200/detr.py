@@ -167,20 +167,54 @@ class DetrEngine:
         return _f32(images, dev), mask
 
     # ------------------------------------------------------------------ DETR.forward
-    def forward(self, samples):
+    def forward(self, samples, aux_loss: bool = False):
         """``DETR.forward`` (DETR/models/detr.py:46-77): {"pred_logits" [B,Q,C+1], "pred_boxes" [B,Q,4]} of the last decoder
-        layer; pred_boxes = sigmoid(bbox_embed(hs)) (:73, MLP :309-321)."""
+        layer; pred_boxes = sigmoid(bbox_embed(hs)) (:73, MLP :309-321).  ``aux_loss=True`` adds "aux_outputs" (:74-75,
+        ``_set_aux_loss`` :95-100): see ``aux_outputs``."""
         feats = self.features(samples)
         self._run(feats, None, backward=False)
         out = {"pred_logits": self.pred_logits}
         if self.bbox_embed:
             out["pred_boxes"] = self._boxes(self.saved["hs"].v)
+        if aux_loss:
+            out["aux_outputs"] = self.aux_outputs()
         return out
 
     __call__ = forward
 
+    def aux_outputs(self) -> List[Dict[str, torch.Tensor]]:
+        """The auxiliary outputs of the last forward: for decoder layers 0 .. L-2, {"pred_logits" [B,Q,C+1], "pred_boxes"
+        [B,Q,4]} of class_embed / sigmoid(bbox_embed) applied to decoder.norm(layer output) (DETR/models/transformer.py:
+        146-151, detr.py:70-77).  The L-1 normalised outputs form one [(L-1) B Q, d] matrix, so the class head and each
+        layer of the box MLP are one GEMM for all of them; the returned tensors are views of the two results."""
+        if not self.bbox_embed:
+            raise MmxError("aux_outputs needs the box head (bbox_embed.*) in the state dict")
+        B, S, Q = self._shape
+        n, d, rows = len(self.decoder) - 1, self.d_model, B * self.queries
+        if n == 0:
+            return []
+        hs = torch.empty(n * rows, d, device=self.device, dtype=torch.float32)
+        l = lib()
+        W = self.class_embed
+        logits = torch.empty(n * rows, W.out_features, device=self.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            for i, L in enumerate(self.decoder[:-1]):
+                t = L.saved["out"].v
+                check(l.mmx_layernorm_fwd(ptr(t), t.stride(0), None, ptr(self.dec_norm[0]), ptr(self.dec_norm[1]),
+                                          ptr(hs[i * rows:]), d, None, None, rows, d, C.c_float(1e-5), current_stream()))
+            check(l.mmx_linear_packed(ptr(hs), d, ptr(W.w), W.in_features, ptr(W.pw), ptr(W.b), None, 0, ptr(logits),
+                                      W.out_features, None, 0, n * rows, W.out_features, W.in_features, current_stream()))
+        boxes = self._mlp_boxes(hs)
+        C1 = W.out_features
+        return [{"pred_logits": logits[i * rows:(i + 1) * rows].view(B, Q, C1),
+                 "pred_boxes": boxes[i * rows:(i + 1) * rows].view(B, Q, 4)} for i in range(n)]
+
     def _boxes(self, hs: torch.Tensor) -> torch.Tensor:
         B, S, Q = self._shape
+        return self._mlp_boxes(hs).view(B, Q, -1)
+
+    def _mlp_boxes(self, hs: torch.Tensor) -> torch.Tensor:
+        """sigmoid(bbox_embed(hs)) for hs [rows, d]: [rows, 4]"""
         l = lib()
         x = hs
         with torch.cuda.device(self.device):
@@ -192,7 +226,7 @@ class DetrEngine:
                                           W.out_features, ptr(y), act, x.shape[0], W.out_features, W.in_features,
                                           current_stream()))
                 x = y
-        return x.view(B, Q, -1)
+        return x
 
     def _mha(self, tape: Tape, m, query: Var, key: Var, value: Var, B, T, S) -> Var:
         """DETR/modules/layers.py:728-768: separate projections, q scaled before q k^T, masks ignored."""
@@ -474,10 +508,11 @@ class MaskGenerator:
     METHODS = ("ours_with_lrp", "ours_no_lrp", "ablation_no_self_in_10", "ablation_no_aggregation", "ours_no_lrp_no_norm",
                "transformer_att", "partial_lrp", "raw_attn", "attn_gradcam", "rollout")
 
-    def __init__(self, model):
+    def __init__(self, model, aux_loss: bool = False):
         self.gen = Generator(model)
         self.abl = GeneratorAlbationNoAgg(self.gen.model)
         self.model = self.gen.model
+        self.aux_loss = bool(aux_loss)
 
     def sample_bytes(self, S: int, lrp: bool) -> int:
         """Device memory one query of a chunk stages at S tokens: A and dA of every attention layer (fp32, rows padded to a
@@ -532,7 +567,9 @@ class MaskGenerator:
         queries go through ``get_masks`` on the same backbone features.  Returns {"pred_logits" [1,Q,C+1], "pred_boxes"
         [1,Q,4], "pred_masks" [1,Q,h,w]} on the device, pred_masks -1 on the dropped queries and the {0, 255} Otsu mask on
         the kept ones.  Prints "no segmentation" when at most one query is kept (:65-66).  An unknown ``method`` prints
-        and returns None before any work; the reference's two shape-probing forwards (:47, :80) are not needed."""
+        and returns None before any work; the reference's two shape-probing forwards (:47, :80) are not needed.  With
+        ``aux_loss=True`` (the reference model built with DETR's default ``aux_loss``) the dict also holds
+        "aux_outputs" (``DetrEngine.aux_outputs``) between "pred_boxes" and "pred_masks", as the reference's does."""
         if method not in self.METHODS:
             print("please provide a valid explainability method")            # mask_generator.py:111-113
             return None
@@ -545,6 +582,7 @@ class MaskGenerator:
             raise MmxError("get_panoptic needs the box head (bbox_embed.*) in the state dict")
         logits = m.pred_logits
         boxes = m._boxes(m.saved["hs"].v)
+        aux = m.aux_outputs() if self.aux_loss else None
         keep = detr_postprocess(logits)["keep"][0]
         q = keep.nonzero().flatten()                                           # one host sync, as keep.nonzero() there
         K, Q, h, w = q.numel(), m.queries, feats.h, feats.w
@@ -554,6 +592,8 @@ class MaskGenerator:
         if K:
             masks, _, _ = self._masks(feats, q, method, max_batch)
             pred_masks.index_copy_(1, q, masks.view(1, K, h, w))
+        if aux is not None:
+            return {"pred_logits": logits, "pred_boxes": boxes, "aux_outputs": aux, "pred_masks": pred_masks}
         return {"pred_logits": logits, "pred_boxes": boxes, "pred_masks": pred_masks}
 
     def _cams(self, batch: _Feats, q: torch.Tensor, method: str) -> torch.Tensor:
