@@ -260,10 +260,15 @@ int tower_forward(Tower& T, int B) {
     GemmEpilogue e2; e2.bias = w.bo; e2.residual = x_in; e2.ldres = D; e2.m_dev = mg;
     MMX_TRY(mm(T.o, D, w.Wo, x_mid, D, Mg, e2, st));
     MMX_TRY(layernorm_fwd(x_mid, D, nullptr, w.ln2_g, w.ln2_b, T.h, D, stt + 2 * M, stt + 3 * M, M, D, 1e-5f, st, md));
-    GemmEpilogue e3; e3.bias = w.bfc; e3.C_act = T.g; e3.act = T.act; e3.m_dev = mg;
+    // fc2 takes act(f).  Where its split pass can apply the activation (backend 3), act(f) never goes through HBM: fc1
+    // stores f only.  Elsewhere fc1's epilogue also stores g = act(f), and fc2 reads g.  Same bits either way.
+    GemmEpilogue e4; e4.bias = w.bproj; e4.residual = x_mid; e4.ldres = D; e4.m_dev = mg; e4.a_act = T.act;
+    const bool act_in_split = gemm_a_act_ok(f, 4 * D, packed_operand(w.Wproj.w, w.Wproj.K, w.Wproj.packed, w.Wproj.N, w.Wproj.K),
+                                            x_out, D, w.Wproj.N, w.Wproj.K, e4);
+    if (!act_in_split) e4.a_act = MMX_ACT_NONE;
+    GemmEpilogue e3; e3.bias = w.bfc; e3.C_act = act_in_split ? nullptr : T.g; e3.act = T.act; e3.m_dev = mg;
     MMX_TRY(mm(T.h, D, w.Wfc, f, 4 * D, Mg, e3, st));
-    GemmEpilogue e4; e4.bias = w.bproj; e4.residual = x_mid; e4.ldres = D; e4.m_dev = mg;
-    MMX_TRY(mm(T.g, 4 * D, w.Wproj, x_out, D, Mg, e4, st));
+    MMX_TRY(mm(act_in_split ? f : T.g, 4 * D, w.Wproj, x_out, D, Mg, e4, st));
   }
   return 0;
 }

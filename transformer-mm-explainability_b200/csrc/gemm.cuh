@@ -4,6 +4,8 @@
 
 namespace mmx {
 
+// In place: C may be the very matrix pre or residual is (same base and row stride; each element is read, then written,
+// by one thread).  Operands that overlap C in any other way are not supported.
 struct GemmEpilogue {
   const float* bias = nullptr;      // [N]: added first
   const float* pre = nullptr;       // [M,N]: multiply by act'(pre)  (dgrad through an activation)
@@ -13,6 +15,9 @@ struct GemmEpilogue {
   float* C_act = nullptr;           // [M,N] (row stride ldc): also store act(C); C_act == C stores act(C) only
   int act = MMX_ACT_NONE;
   const int* m_dev = nullptr;       // optional device-resident row count (<= M): M becomes an upper bound (ragged batches)
+  // Not an epilogue: the product takes act(A) for A.  Only the fp16x3 pre-split path (backend 3) applies it, in its split
+  // pass; gemm_nt_b fails on any other path (gemm_a_act_ok says in advance).
+  int a_act = MMX_ACT_NONE;
 };
 
 // A K-major GEMM "B" operand [N,K]: the fp32 matrix and, for static weights, its fp16 hi / lo planes
@@ -38,6 +43,8 @@ int gemm_nt(const float* A, int lda, const float* Bt, int ldb, float* C, int ldc
 // hi / lo planes and the shape qualifies; everything else goes through gemm_nt's rule.
 int gemm_nt_b(const float* A, int lda, const BOperand& B, float* C, int ldc, int M, int N, int K, const GemmEpilogue& ep,
               cudaStream_t st);
+// Whether gemm_nt_b takes this product with ep.a_act set (backend 3 and a shape its fp16x3 kernel accepts).
+bool gemm_a_act_ok(const float* A, int lda, const BOperand& B, float* C, int ldc, int N, int K, const GemmEpilogue& ep);
 
 // fp16x3 backends (gemm_wgmma.cu)
 size_t pack_f16x3_bytes(int N, int K);                 // bytes of one packed operand (hi plane then lo plane)

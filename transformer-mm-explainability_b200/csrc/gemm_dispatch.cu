@@ -45,9 +45,17 @@ int gemm_backend() {
   return b;
 }
 
+bool gemm_a_act_ok(const float* A, int lda, const BOperand& B, float* C, int ldc, int N, int K, const GemmEpilogue& ep) {
+  return gemm_backend() == 3 && B.hi && gemm_f16x3_shape_ok(A, lda, B, C, ldc, N, K, ep);
+}
+
 static int gemm_nt_impl(const float* A, int lda, const BOperand& B, float* C, int ldc, int M, int N, int K,
                         const GemmEpilogue& ep, cudaStream_t st) {
   const int be = gemm_backend();
+  if (ep.a_act != MMX_ACT_NONE) {
+    MMX_REQUIRE(gemm_a_act_ok(A, lda, B, C, ldc, N, K, ep), "an activation on A needs the fp16x3 pre-split backend");
+    return gemm_nt_f16x3(A, lda, B, C, ldc, M, N, K, ep, st, true);
+  }
   if (be >= 2 && B.hi && gemm_f16x3_shape_ok(A, lda, B, C, ldc, N, K, ep)) return gemm_nt_f16x3(A, lda, B, C, ldc, M, N, K, ep, st, be == 3);
   if (be >= 1 && gemm_tc_shape_ok(A, lda, B.w, B.ldw, C, ldc, N, K, ep)) return gemm_nt_tc(A, lda, B.w, B.ldw, C, ldc, M, N, K, ep, st);
   return gemm_nt_simt(A, lda, B.w, B.ldw, C, ldc, M, N, K, ep, st);
@@ -113,6 +121,7 @@ int gemm_nt_b(const float* A, int lda, const BOperand& Bop, float* C, int ldc, i
 
 int gemm_nt_planes(const uint16_t* Ahi, const uint16_t* Alo, int ldpa, const BOperand& B, float* C, int ldc, int M, int N, int K,
                    const GemmEpilogue& ep, cudaStream_t st) {
+  MMX_REQUIRE(ep.a_act == MMX_ACT_NONE, "an activation on A needs the fp16x3 pre-split backend");
   return profiled(M, N, K, ep, st, [&] { return gemm_nt_f16x3_planes(Ahi, Alo, ldpa, B, C, ldc, M, N, K, ep, st); });
 }
 

@@ -144,8 +144,7 @@ __global__ void __launch_bounds__(THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant__ CUtensorMap map1,
                   const __grid_constant__ CUtensorMap map2, const __grid_constant__ CUtensorMap map3, Params p) {
   using cfg = Cfg<MODE, BN>;
-  constexpr int STAGES = cfg::STAGES, STAGE = cfg::STAGE, BK = cfg::BK, ACC = cfg::ACC;
-  extern __shared__ uint8_t smem_raw[];
+  constexpr int STAGES = cfg::STAGES, STAGE = cfg::STAGE, BK = cfg::BK, ACC = cfg::ACC;  extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;      // swizzle-128B tiles need 1024 B alignment
   uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
   const uint32_t bar_base = smem_base + STAGES * STAGE;
@@ -262,37 +261,61 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constan
     }
 
     // ------------------------------------------------------------------ epilogue from the accumulator fragments:
-    // register 4j + 2h + e holds row 16 (warp % 4) + lane / 4 + 8h, column 8j + 2 (lane % 4) + e of the warpgroup's block
+    // register 4j + 2h + e holds row 16 (warp % 4) + lane / 4 + 8h, column 8j + 2 (lane % 4) + e of the warpgroup's block.
+    // C, pre and residual may alias, so a load written after a store cannot be issued before it: every load of the
+    // fragment is written first, into the cross accumulator once it is folded, and the stores come last.  The tile then
+    // waits for one memory round trip (two with pre and residual: pre goes first), not one per stored row pair.
+    // Arithmetic order per element: fold, + bias, * act'(pre), + residual, store, act(C).
     const int mrow = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2), cq = 2 * (lane & 3);
     const long long c_off = bi * p.stride_c, r_off = bi * p.stride_res;
+    // N % 4 == 0: a column pair is inside or outside
+    auto inside = [&](int j, int h) { return n0 + 8 * j + cq < p.N && mrow + 8 * h < p.M; };
+    auto load_frag = [&](const float* base, int ld) {            // crs <- base's elements of the thread's fragment
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (inside(j, h)) {
+            const float2 x = *reinterpret_cast<const float2*>(base + (long long)(mrow + 8 * h) * ld + n0 + 8 * j + cq);
+            crs[4 * j + 2 * h] = x.x; crs[4 * j + 2 * h + 1] = x.y;
+          }
+    };
+#pragma unroll
+    for (int i = 0; i < ACC; ++i) {
+      if constexpr (MODE == TF32X3) acc[i] = acc[i] + crs[i];
+      else acc[i] = fmaf(crs[i], LO_INV, acc[i]);
+    }
+    if (p.ep.bias) {
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int n = n0 + 8 * j + cq;
+        if (n >= p.N) continue;
+        const float2 b = __ldg(reinterpret_cast<const float2*>(p.ep.bias + n));
+        acc[4 * j] += b.x; acc[4 * j + 1] += b.y; acc[4 * j + 2] += b.x; acc[4 * j + 3] += b.y;
+      }
+    }
+    if (ACT && p.ep.pre) {
+      load_frag(p.ep.pre, p.ep.ldpre);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (inside(j, h)) {
+            const int i = 4 * j + 2 * h;
+            const float2 f = act_bwd2(make_float2(crs[i], crs[i + 1]), p.ep.act);
+            acc[i] *= f.x; acc[i + 1] *= f.y;
+          }
+    }
+    if (p.ep.residual) load_frag(p.ep.residual + r_off, p.ep.ldres);
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
       const int n = n0 + 8 * j + cq;
-      if (n >= p.N) continue;                                    // N % 4 == 0: a column pair is inside or outside
-      float2 b = make_float2(0.f, 0.f);
-      if (p.ep.bias) b = __ldg(reinterpret_cast<const float2*>(p.ep.bias + n));
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int m = mrow + 8 * h;
-        if (m >= p.M) continue;
-        const int i = 4 * j + 2 * h;
-        float2 v;
-        if constexpr (MODE == TF32X3) {
-          v.x = acc[i] + crs[i];
-          v.y = acc[i + 1] + crs[i + 1];
-        } else {
-          v.x = fmaf(crs[i], LO_INV, acc[i]);
-          v.y = fmaf(crs[i + 1], LO_INV, acc[i + 1]);
-        }
-        v.x += b.x; v.y += b.y;
-        if (ACT && p.ep.pre) {
-          const float2 f = act_bwd2(*reinterpret_cast<const float2*>(p.ep.pre + (long long)m * p.ep.ldpre + n), p.ep.act);
-          v.x *= f.x; v.y *= f.y;
-        }
-        if (p.ep.residual) {
-          const float2 a = *reinterpret_cast<const float2*>(p.ep.residual + r_off + (long long)m * p.ep.ldres + n);
-          v.x += a.x; v.y += a.y;
-        }
+        if (!inside(j, h)) continue;
+        const int m = mrow + 8 * h, i = 4 * j + 2 * h;
+        float2 v = make_float2(acc[i], acc[i + 1]);
+        if (p.ep.residual) { v.x += crs[i]; v.y += crs[i + 1]; }
         if (!ACT || p.ep.C_act != p.C) *reinterpret_cast<float2*>(p.C + c_off + (long long)m * p.ldc + n) = v;
         if (ACT && p.ep.C_act) *reinterpret_cast<float2*>(p.ep.C_act + (long long)m * p.ldc + n) = act_fwd2(v, p.ep.act);
       }
@@ -300,10 +323,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constan
   }
 }
 
-// fp32 A [M, K] (row stride lda, lda % 4 == 0) -> hi / lo' fp16 planes [M, ldp]; 4 elements per thread.  Columns K .. ldp-1
-// are never read (the tensor maps declare K columns, TMA zero-fills beyond).
+// act(fp32 A) [M, K] (row stride lda, lda % 4 == 0) -> hi / lo' fp16 planes [M, ldp]; 4 elements per thread.  Columns
+// K .. ldp-1 are never read (the tensor maps declare K columns, TMA zero-fills beyond).  act goes through the epilogue's
+// act_fwd2, so act(A) here has the bits a C_act store of the GEMM that produced A would have had.
 __global__ void __launch_bounds__(256) split_a_planes_kernel(const float* __restrict__ A, int lda, __half* __restrict__ hi,
-                                                             __half* __restrict__ lo, int ldp, int M, int K) {
+                                                             __half* __restrict__ lo, int ldp, int M, int K, int act) {
   const int kc = (K + 3) / 4;
   const long long total = (long long)M * kc;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -312,6 +336,10 @@ __global__ void __launch_bounds__(256) split_a_planes_kernel(const float* __rest
     float4 x;
     if (k + 4 <= K) x = *reinterpret_cast<const float4*>(src);
     else { x.x = src[0]; x.y = k + 1 < K ? src[1] : 0.f; x.z = k + 2 < K ? src[2] : 0.f; x.w = 0.f; }
+    if (act != MMX_ACT_NONE) {
+      const float2 a = act_fwd2(make_float2(x.x, x.y), act), b = act_fwd2(make_float2(x.z, x.w), act);
+      x = make_float4(a.x, a.y, b.x, b.y);
+    }
     uint2 h, l;
     split2(x.x, x.y, h.x, l.x);
     split2(x.z, x.w, h.y, l.y);
@@ -438,7 +466,7 @@ static int gemm_presplit(const float* A, int lda, const BOperand& B, const Param
   __half *Ahi = planes, *Alo = planes + (size_t)M * ldpa;
   const long long total = (long long)M * ((K + 3) / 4);
   const int grid = (int)((total + 255) / 256 < (long long)sm_count() * 8 ? (total + 255) / 256 : (long long)sm_count() * 8);
-  split_a_planes_kernel<<<grid, 256, 0, st>>>(A, lda, Ahi, Alo, ldpa, M, K);
+  split_a_planes_kernel<<<grid, 256, 0, st>>>(A, lda, Ahi, Alo, ldpa, M, K, p.ep.a_act);
   MMX_LAUNCH_CHECK();
   const int rc = gemm_planes(Ahi, Alo, ldpa, B, p, st);
   cudaFreeAsync(planes, st);
