@@ -349,7 +349,12 @@ int mmx_clip_interpret_host(mmx_clip* h, const float* images, int n_images, cons
 int mmx_clip_set_serial(mmx_clip* h, int serial);
 
 /* Test taps: device pointers into the engine workspace after the last interpret (valid for batch <= max_batch,
- * first micro-batch).  what: "A" / "dA" / "Abar" (tower 0 = vision, 1 = text, layer index), "logits" ([B,B]).
+ * first micro-batch).  what: "A" / "dA" ([B,H,S,S]) / "Abar" ([B,S,S]) (tower 0 = vision, 1 = text, layer index),
+ * "logits" ([B,B]); the residual stream "x" ([M,D], layer 0 .. L: x of layer l is the input of block l, layer L the tower
+ * output), "xmid" ([M,D]), "qkv" ([M,3D]), "f" ([M,4D], fc1 before the activation) and "stats" ([4,M]: mean1, rstd1,
+ * mean2, rstd2 of the block's two LayerNorms) of block `layer`; per tower, `layer` ignored: "feat", "featn", "dfeat"
+ * ([B,E]: pooled features, their normalised copy, the seed gradient times gscale) and "gscale" ([B]).  M = B*S rows, except
+ * for the ragged text tower: its rows are packed and M is the packed row count of the last call.
  * Writes the pointer, the dims (up to 4) and the row stride of the last dim. */
 int mmx_clip_tap(mmx_clip* h, const char* what, int tower, int layer, const float** ptr, int dims[4], int* ld);
 
@@ -361,6 +366,38 @@ int mmx_attention_bwd_scaled(const float* dO, int lddo, const float* Q, int ldq,
                              const float* V, int ldv, const float* A, float* dA, int ldA, float* delta,
                              float* dQ, int lddq, float* dK, int lddk, float* dV, int lddv,
                              int B, int H, int T, int S, int hd, float scale, int flags, const float* gscale, void* stream);
+
+/* Ragged self-attention, the CLIP text tower's packed rows: sample b owns rows offs[b] .. offs[b] + lens[b] - 1 of Q / K / V
+ * / O (and of dO / dQ / dK / dV) and attends within them only (T = S = lens[b], 1 <= lens[b] <= T).  offs, lens: [B] device
+ * ints (mmx_text_embed_packed writes them).  The staged A / dA planes stay dense [B,H,T,ldA]: rows and columns >= lens[b] are
+ * written as 0.  Packed rows past sum(lens) are neither read nor written.  T <= 1024 and no key bias; otherwise as
+ * mmx_attention_fwd / mmx_attention_bwd_scaled (gscale may be NULL; dQ / dK / dV all NULL stops after dA). */
+int mmx_attention_fwd_ragged(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv, float* A, int ldA,
+                             float* O, int ldo, const int* offs, const int* lens, int B, int H, int T, int hd, float scale,
+                             int flags, void* stream);
+int mmx_attention_bwd_ragged(const float* dO, int lddo, const float* Q, int ldq, const float* K, int ldk, const float* V,
+                             int ldv, const float* A, float* dA, int ldA, float* delta, float* dQ, int lddq, float* dK,
+                             int lddk, float* dV, int lddv, const int* offs, const int* lens, int B, int H, int T, int hd,
+                             float scale, int flags, const float* gscale, void* stream);
+
+/* The CLIP engine's token assembly and logit head as standalone calls (row-major, dense rows). */
+/* Packed text embedding (CLIP/clip/model.py:350-352,360): lens[b] = 1 + the first argmax of tokens[b, 0:S] (the EOT; rows
+ * after it cannot reach the pooled feature under the causal mask), offs = exclusive scan of lens, eot_row[b] = offs[b] +
+ * lens[b] - 1, *total = sum(lens); x[offs[b] + s] = emb[tokens[b,s]] + pos[s] for s < lens[b] (token ids clamped to
+ * [0, vocab)).  tokens: [B,S] int32, emb: [vocab,D], pos: [S,D], x: [B*S,D] (rows past *total untouched); all device. */
+int mmx_text_embed_packed(const int32_t* tokens, const float* emb, const float* pos, float* x, int* offs, int* lens,
+                          int* eot_row, int* total, int B, int S, int D, int vocab, void* stream);
+/* Vision tokens with the ln_pre fused (CLIP/clip/model.py:233-235): x[b,0] = LN(cls + pos[0]), x[b,1+g] =
+ * LN(patch_emb[(b % n_img)*(S-1) + g] + pos[1+g]).  patch_emb: [n_img*(S-1),D], pos: [S,D], x: [B*S,D]. */
+int mmx_vision_tokens_lnpre(const float* patch_emb, int n_img, const float* cls, const float* pos, const float* gamma,
+                            const float* beta, float* x, int B, int S, int D, float eps, void* stream);
+/* Logit head and its analytic backward for y = sum_b logits_per_image[b,b] (CLIP/clip/model.py:368-374,
+ * CLIP_explainability.ipynb:156-160), one warp per sample: fin / ftn = fi / |fi|, ft / |ft|; diag[b] = logit_scale_exp *
+ * <fin_b, ftn_b> (diag may be NULL); dfi / dft = dy / d(fi, ft).  With gs_i / gs_t given, row b of dfi (dft) is multiplied
+ * by the power of two gs_i[b] (gs_t[b]) that puts its max |.| in [16, 32) (1 when that max is 0 or not finite), and the
+ * factors are written.  fi, ft, fin, ftn, dfi, dft: [B,E]. */
+int mmx_clip_head(const float* fi, const float* ft, float logit_scale_exp, float* fin, float* ftn, float* dfi, float* dft,
+                  float* diag, float* gs_i, float* gs_t, int B, int E, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * LRP (`relprop`) primitives: the second sweep behind use_lrp=True / generate_transformer_att / generate_partial_lrp

@@ -100,7 +100,20 @@ _SIGS = {
                                            c_float_p, c_float_p, C.c_int, c_float_p, c_float_p, C.c_int, c_float_p, C.c_int,
                                            c_float_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int,
                                            c_float_p, C.c_void_p]),
-    "mmx_conv2d": (C.c_int, [c_float_p] + [C.c_longlong] * 4 + [C.c_int] * 4 + [c_float_p, C.c_int, C.c_void_p, c_float_p,
+    "mmx_attention_fwd_ragged": (C.c_int, [c_float_p, C.c_int, c_float_p, C.c_int, c_float_p, C.c_int, c_float_p, C.c_int,
+                                           c_float_p, C.c_int, c_int_p, c_int_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                           C.c_int, C.c_void_p]),
+    "mmx_attention_bwd_ragged": (C.c_int, [c_float_p, C.c_int, c_float_p, C.c_int, c_float_p, C.c_int, c_float_p, C.c_int,
+                                           c_float_p, c_float_p, C.c_int, c_float_p, c_float_p, C.c_int, c_float_p, C.c_int,
+                                           c_float_p, C.c_int, c_int_p, c_int_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                           C.c_int, c_float_p, C.c_void_p]),
+    "mmx_text_embed_packed": (C.c_int, [c_int_p, c_float_p, c_float_p, c_float_p, c_int_p, c_int_p, c_int_p, c_int_p,
+                                        C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "mmx_vision_tokens_lnpre": (C.c_int, [c_float_p, C.c_int, c_float_p, c_float_p, c_float_p, c_float_p, c_float_p,
+                                          C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]),
+    "mmx_clip_head": (C.c_int, [c_float_p, c_float_p, C.c_float, c_float_p, c_float_p, c_float_p, c_float_p, c_float_p,
+                                c_float_p, c_float_p, C.c_int, C.c_int, C.c_void_p]),
+    "mmx_conv2d":(C.c_int, [c_float_p] + [C.c_longlong] * 4 + [C.c_int] * 4 + [c_float_p, C.c_int, C.c_void_p, c_float_p,
                                                                               c_float_p, C.c_int, c_float_p, C.c_int]
                    + [C.c_int] * 6 + [C.c_void_p]),
     "mmx_conv2d_dilated": (C.c_int, [c_float_p] + [C.c_longlong] * 4 + [C.c_int] * 4 + [c_float_p, C.c_int, C.c_void_p, c_float_p,

@@ -157,14 +157,22 @@ class ClipEngine:
         return out
 
     def tap(self, what: str, tower: int = 0, layer: int = 0) -> torch.Tensor:
-        """Copy of an intermediate of the last interpret call: 'A', 'dA' [B,H,S,S], 'Abar' [B,S,S], 'logits' [B,B]."""
+        """Copy of an intermediate of the last interpret call (tower 0 = vision, 1 = text):
+        - of block ``layer``: 'A', 'dA' [B,H,S,S], 'Abar' [B,S,S], 'xmid' [M,D], 'qkv' [M,3D], 'f' [M,4D] (fc1 before
+          the activation), 'stats' [4,M] (mean1, rstd1, mean2, rstd2); 'x' [M,D] for layer 0 .. L (the input of block
+          ``layer``; layer L is the tower output);
+        - of the tower (``layer`` ignored): 'feat', 'featn', 'dfeat' [B,E] (dfeat carries the factor gscale), 'gscale' [B];
+        - 'logits' [B,B].
+        M = B*S, except for the ragged text tower: its rows are packed, sample b's at offs[b] .. offs[b] + len[b] - 1
+        (len[b] = first argmax of its tokens + 1), and M = sum(len) of the last call."""
         p = C.c_void_p()
         dims = (C.c_int * 4)()
         ld = C.c_int()
         check(self._lib.mmx_clip_tap(self._h, what.encode(), tower, layer, C.byref(p), C.byref(dims), C.byref(ld)))
         shape = [d for d in dims]
         n_lead = 1
-        nd = {"A": 4, "dA": 4, "Abar": 3, "logits": 2}[what]
+        nd = {"A": 4, "dA": 4, "Abar": 3, "logits": 2, "x": 2, "xmid": 2, "qkv": 2, "f": 2, "stats": 2, "feat": 2, "featn": 2,
+              "dfeat": 2, "gscale": 1}[what]
         shape = shape[:nd]
         for d in shape[:-1]:
             n_lead *= d

@@ -1394,4 +1394,19 @@ int mmx_attention_bwd_scaled(const float* dO, int lddo, const float* Q, int ldq,
   return attention_bwd(dO, lddo, Q, ldq, K, ldk, V, ldv, A, dA, ldA, delta, dQ, lddq, dK, lddk, dV, lddv, B, H, T, S, hd, scale,
                        flags, (cudaStream_t)stream, nullptr, nullptr, gscale);
 }
+int mmx_attention_fwd_ragged(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv, float* A, int ldA,
+                             float* O, int ldo, const int* offs, const int* lens, int B, int H, int T, int hd, float scale,
+                             int flags, void* stream) {
+  MMX_REQUIRE(offs != nullptr && lens != nullptr, "ragged attention needs offs and lens");
+  return attention_fwd(Q, ldq, K, ldk, V, ldv, nullptr, A, ldA, O, ldo, B, H, T, T, hd, scale, flags, (cudaStream_t)stream, offs,
+                       lens);
+}
+int mmx_attention_bwd_ragged(const float* dO, int lddo, const float* Q, int ldq, const float* K, int ldk, const float* V,
+                             int ldv, const float* A, float* dA, int ldA, float* delta, float* dQ, int lddq, float* dK,
+                             int lddk, float* dV, int lddv, const int* offs, const int* lens, int B, int H, int T, int hd,
+                             float scale, int flags, const float* gscale, void* stream) {
+  MMX_REQUIRE(offs != nullptr && lens != nullptr, "ragged attention needs offs and lens");
+  return attention_bwd(dO, lddo, Q, ldq, K, ldk, V, ldv, A, dA, ldA, delta, dQ, lddq, dK, lddk, dV, lddv, B, H, T, T, hd, scale,
+                       flags, (cudaStream_t)stream, offs, lens, gscale);
+}
 }

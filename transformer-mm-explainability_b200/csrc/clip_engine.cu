@@ -653,8 +653,37 @@ int mmx_clip_tap(mmx_clip* h, const char* what, int tower, int layer, const floa
     *ptr = h->logits; dims[0] = B; dims[1] = B; dims[2] = dims[3] = 1; *ld = B;
     return 0;
   }
+  MMX_REQUIRE(tower == 0 || tower == 1, "tower must be 0 (vision) or 1 (text)");
   Tower& T = tower == 0 ? h->v : h->t;
+  const int E = h->E;
+  if (w == "feat" || w == "featn" || w == "dfeat") {
+    *ptr = w == "feat" ? T.feat : (w == "featn" ? T.featn : T.dfeat);
+    dims[0] = B; dims[1] = E; dims[2] = dims[3] = 1; *ld = E;
+    return 0;
+  }
+  if (w == "gscale") {
+    *ptr = T.gscale; dims[0] = B; dims[1] = dims[2] = dims[3] = 1; *ld = B;
+    return 0;
+  }
+  // activation arena: layer stride B*S rows; a ragged tower's live rows are the first rows_host of each layer
+  const size_t M = (size_t)T.M(B), MD = M * T.D;
+  const int rows = (T.ragged && T.rows_host >= 0) ? T.rows_host : (int)M;
+  if (w == "x") {
+    MMX_REQUIRE(layer >= 0 && layer <= T.L, "layer out of range");
+    *ptr = T.x + layer * MD; dims[0] = rows; dims[1] = T.D; dims[2] = dims[3] = 1; *ld = T.D;
+    return 0;
+  }
   MMX_REQUIRE(layer >= 0 && layer < T.L, "layer out of range");
+  if (w == "xmid" || w == "qkv" || w == "f") {
+    const int n = w == "xmid" ? 1 : (w == "qkv" ? 3 : 4);
+    *ptr = (w == "xmid" ? T.xmid : (w == "qkv" ? T.qkv : T.f)) + layer * MD * n;
+    dims[0] = rows; dims[1] = n * T.D; dims[2] = dims[3] = 1; *ld = n * T.D;
+    return 0;
+  }
+  if (w == "stats") {
+    *ptr = T.stats + (size_t)layer * 4 * M; dims[0] = 4; dims[1] = rows; dims[2] = dims[3] = 1; *ld = (int)M;
+    return 0;
+  }
   const size_t plane = (size_t)B * T.H * T.S * T.ld;
   if (w == "A" || w == "dA") {
     *ptr = (w == "A" ? T.A : T.dA) + layer * plane;

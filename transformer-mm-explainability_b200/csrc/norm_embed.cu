@@ -543,4 +543,21 @@ int mmx_layernorm_bwd(const float* dy, int lddy, const float* x, int ldx, const 
   return layernorm_bwd(dy, lddy, x, ldx, row_map, gamma, mean, rstd, residual_grad, ldres, dx, lddx, rows, D,
                        (cudaStream_t)stream, nullptr);
 }
+int mmx_text_embed_packed(const int32_t* tokens, const float* emb, const float* pos, float* x, int* offs, int* lens,
+                          int* eot_row, int* total, int B, int S, int D, int vocab, void* stream) {
+  MMX_REQUIRE(B > 0 && S > 0 && D > 0 && vocab > 0, "bad sizes");
+  return text_embed_packed(tokens, emb, pos, x, offs, lens, eot_row, total, B, S, D, vocab, (cudaStream_t)stream);
+}
+int mmx_vision_tokens_lnpre(const float* patch_emb, int n_img, const float* cls, const float* pos, const float* gamma,
+                            const float* beta, float* x, int B, int S, int D, float eps, void* stream) {
+  MMX_REQUIRE(B > 0 && S > 1 && D > 0 && n_img > 0, "bad sizes");
+  return vision_tokens_lnpre(patch_emb, n_img, cls, pos, gamma, beta, x, B, S, D, eps, (cudaStream_t)stream);
+}
+int mmx_clip_head(const float* fi, const float* ft, float logit_scale_exp, float* fin, float* ftn, float* dfi, float* dft,
+                  float* diag, float* gs_i, float* gs_t, int B, int E, void* stream) {
+  MMX_REQUIRE(B > 0 && E > 0, "bad sizes");
+  MMX_REQUIRE(fi && ft && fin && ftn && dfi && dft, "fi, ft, fin, ftn, dfi and dft are required");
+  MMX_REQUIRE((gs_i == nullptr) == (gs_t == nullptr), "gs_i / gs_t: both or neither");
+  return clip_head(fi, ft, logit_scale_exp, fin, ftn, dfi, dft, diag, gs_i, gs_t, B, E, (cudaStream_t)stream);
+}
 }
