@@ -96,9 +96,11 @@ def generate_ours(sd, cfg: DetrConfig, src, pos, target_index, index=None, norma
     G_e, G_ds, G_dc = grads[:ne], grads[ne:ne + nd], grads[ne + nd:]
     S, Q = A_e[0].shape[-1], A_ds[0].shape[-1]
     out = []
+    dev = src.device
     for b in range(B):
         sl = slice(b * H, (b + 1) * H)
-        R_ii, R_qq, R_qi = torch.eye(S, dtype=dtype), torch.eye(Q, dtype=dtype), torch.zeros(Q, S, dtype=dtype)
+        R_ii, R_qq = torch.eye(S, dtype=dtype, device=dev), torch.eye(Q, dtype=dtype, device=dev)
+        R_qi = torch.zeros(Q, S, dtype=dtype, device=dev)
         for A, G in zip(A_e, G_e):                                                   # :110-118
             R_ii = R_ii + R_.avg_heads(A[sl].detach(), G[sl]) @ R_ii
         for A, G, Ac, Gc in zip(A_ds, G_ds, A_dc, G_dc):

@@ -95,11 +95,12 @@ def lxmert_forward(sd, cfg: LxmertConfig, ids, feats, boxes, lang_mask=None, vis
 
 
 def generate_ours(sd, cfg: LxmertConfig, ids, feats, boxes, index=None, normalize_self_attention=True,
-                  apply_self_in_rule_10=True, dtype=torch.float32):
-    """GeneratorOurs.generate_ours(use_lrp=False) per sample.  Returns (R_t_t [B,T,T], R_t_i [B,T,I], logits)."""
+                  apply_self_in_rule_10=True, dtype=torch.float32, lang_mask=None, vis_mask=None):
+    """GeneratorOurs.generate_ours(use_lrp=False) per sample, with LxmertForQuestionAnswering's attention_mask /
+    visual_attention_mask as ``lang_mask`` / ``vis_mask``.  Returns (R_t_t [B,T,T], R_t_i [B,T,I], logits)."""
     sd = {k: v.detach().to(dtype).requires_grad_(True) for k, v in sd.items()}
     feats, boxes = feats.to(dtype), boxes.to(dtype)
-    logits, st = lxmert_forward(sd, cfg, ids, feats, boxes)
+    logits, st = lxmert_forward(sd, cfg, ids, feats, boxes, lang_mask, vis_mask)
     B, T = ids.shape
     I = feats.shape[1]
     idx = logits.argmax(-1) if index is None else torch.as_tensor(index).reshape(B)
@@ -114,10 +115,11 @@ def generate_ours(sd, cfg: LxmertConfig, ids, feats, boxes, index=None, normaliz
     nx = cfg.x_layers
     norm, s10 = normalize_self_attention, apply_self_in_rule_10
     Rtt, Rti = [], []
+    dev = feats.device
     for b in range(B):
         cam = lambda n, i: R_.avg_heads(st[n][i][b].detach(), G[n][i][b])
-        R_tt, R_ii = torch.eye(T, dtype=dtype), torch.eye(I, dtype=dtype)
-        R_ti, R_it = torch.zeros(T, I, dtype=dtype), torch.zeros(I, T, dtype=dtype)
+        R_tt, R_ii = torch.eye(T, dtype=dtype, device=dev), torch.eye(I, dtype=dtype, device=dev)
+        R_ti, R_it = torch.zeros(T, I, dtype=dtype, device=dev), torch.zeros(I, T, dtype=dtype, device=dev)
         for i in range(cfg.l_layers):                                               # EG:61-71
             a, c = R_.apply_self_attention_rules(R_tt, R_ti, cam("lang", i)); R_tt, R_ti = R_tt + a, R_ti + c
         for i in range(cfg.r_layers):                                               # EG:73-83

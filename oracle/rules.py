@@ -36,7 +36,7 @@ def handle_residual(orig_self_attention: torch.Tensor) -> torch.Tensor:
     """Eq. 8-9.  DETR/modules/ExplanationGenerator.py:46-53: ``(R-I)/rowsum(R-I) + I`` with the
     ``diag(R-I) >= 0`` assertion (AssertionError on violation, like the reference)."""
     n = orig_self_attention.shape[-1]
-    eye = torch.eye(n, dtype=orig_self_attention.dtype)
+    eye = torch.eye(n, dtype=orig_self_attention.dtype, device=orig_self_attention.device)
     sa = orig_self_attention.clone() - eye
     assert sa.diagonal().min() >= 0
     sa = sa / sa.sum(dim=-1, keepdim=True)

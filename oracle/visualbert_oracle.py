@@ -157,7 +157,7 @@ def generate_ours(sd, cfg, inp, index=None, dtype=torch.float32):
     idx = scores.argmax(-1) if index is None else torch.as_tensor(index).reshape(-1).expand(B)
     grads = torch.autograd.grad(scores[torch.arange(B), idx].sum(), st)
     S = st[0].shape[-1]
-    R = torch.eye(S, dtype=dtype).repeat(B, 1, 1)
+    R = torch.eye(S, dtype=dtype, device=scores.device).repeat(B, 1, 1)
     for A, G in zip(st, grads):
         cam = (G * A.detach()).clamp(min=0).mean(dim=1)
         R = R + torch.bmm(cam, R)

@@ -104,7 +104,7 @@ def generate_relevance(sd, cfg: VitConfig, images, index=None, dtype=torch.float
     out = []
     for b in range(B):
         S = stage[0].shape[-1]
-        R = torch.eye(S, dtype=dtype)
+        R = torch.eye(S, dtype=dtype, device=images.device)
         for A, G in zip(stage, grads):
             cam = avg_heads(A[b].detach(), G[b])
             R = R + cam @ R

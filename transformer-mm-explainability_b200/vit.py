@@ -82,6 +82,7 @@ class ViTEngine:
             xn = tape.layernorm(tape.gather_rows(x, rows_cls), *self.norm, 1e-6)
             logits = tape.linear(xn, self.head)
             self.logits = logits.v
+            self.saved = dict(B=B, xn=xn)
             idx = logits.v.argmax(-1) if index is None else torch.as_tensor(index, device=self.device).reshape(B)
             one_hot = torch.zeros_like(logits.v)
             one_hot.scatter_(1, idx.long().reshape(B, 1), 1.0)                   # ipynb:1186-1190
