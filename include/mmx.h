@@ -489,6 +489,32 @@ int mmx_detr_mask_losses(const float* pred_masks, int B, int Q, int h, int w, co
                          int mask_dtype, const int* tgt_offsets, const int64_t* indices, const float* num_boxes, float* out,
                          void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * Visualisation: the notebooks' last step, a relevance map turned into the picture a person looks at.  One launch per
+ * call (one thread-block cluster per picture), no host synchronisation, no float atomics: deterministic and capturable.
+ * ------------------------------------------------------------------------------------------------------- */
+/* show_image_relevance (CLIP_explainability.ipynb:216) and generate_visualization (Transformer_MM_explainability_ViT.ipynb
+ * :1223,1234): rel [B, h*w] fp32, images [n_img in {1, B}, 3, H, W] fp32 NCHW, out [B, H, W, 3] uint8.  Per map:
+ * F.interpolate(bilinear, align_corners=False) to H x W with ATen's CUDA arithmetic (source scales scale_h / scale_w:
+ * 1 / scale_factor, or (float)in / out for a size), a copy when the sizes are equal; min-max of the map and of the image
+ * (all three channels); q = uint8(255 m) (truncation, NaN -> 0); cam = JET[q] / 255 + img, BGR channel c with RGB
+ * channel c; vis = cam / max(cam) (NaN propagates); out = uint8(255 vis) with RGB <-> BGR swapped (cv2.cvtColor).
+ * The JET table is cv2's COLORMAP_JET, held in the library.  h * w <= 4096 unless (h, w) = (H, W). */
+int mmx_relevance_overlay(const float* rel, int B, int h, int w, float scale_h, float scale_w, const float* images, int n_img,
+                          int H, int W, unsigned char* out, void* stream);
+/* save_image_vis (LXMERT.ipynb:121, Transformer_MM_Explainability.ipynb:2571): img [n_img in {1, B}, H, W, 3] uint8 BGR,
+ * boxes [B, n_boxes, 4] fp32 pixels (x0, y0, x1, y1), scores [B, n_boxes], out [B, H, W, 3] uint8 (what cv2.imwrite
+ * encodes).  Box i covers mask[int(y0):int(y1), int(x0):int(x1)] with Python slice rules (truncation, one wrap of a
+ * negative bound, clamping, start >= stop empty) and sets it to torch.max(score, mask) (NaN propagates); the mask is
+ * min-max normalised in fp32 and multiplied into the image; the product goes to 8 bits as OpenCV's convertTo does (round
+ * half to even, saturate, NaN -> 0).  n_boxes <= 1024. */
+int mmx_box_relevance_image(const unsigned char* img, int n_img, int H, int W, const float* boxes, const float* scores, int B,
+                            int n_boxes, unsigned char* out, void* stream);
+/* show_heatmap_on_text's text_scores (CLIP_explainability.ipynb:254): R_text [B, ctx, ctx], tokens [B, ctx] int32.
+ * eot = first argmax of tokens[b]; lens[b] = max(eot - 1, 0); scores[b, j] = R_text[b, eot, 1 + j] / s for j < lens[b]
+ * (0 beyond), s the slice's sum in double rounded once to fp32.  scores [B, ctx] fp32, lens [B] int32, both device. */
+int mmx_clip_text_scores(const float* R_text, const int* tokens, int B, int ctx, float* scores, int* lens, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -4,6 +4,8 @@ Host-side mirror of the reference's Python API (hila-chefer/Transformer-MM-Expla
 libmmx.so (include/mmx.h).  Names, argument meaning and error behaviour follow the reference:
 
   * ``interpret(image, texts, model, device, start_layer=-1, start_layer_text=-1)``  - CLIP_explainability.ipynb cell 6
+  * ``show_image_relevance``, ``generate_visualization``, ``save_image_vis``, ``show_heatmap_on_text``  - the notebooks'
+    visualisation step, returning device tensors (``visualize.py``)
   * ``avg_heads``, ``apply_self_attention_rules``, ``apply_mm_attention_rules``, ``handle_residual``,
     ``compute_rollout_attention``  - DETR/modules/ExplanationGenerator.py:5-53, lxmert/lxmert/src/ExplanationGenerator.py:5-54
 
@@ -24,6 +26,7 @@ from .backbone import DetrBackbone  # noqa: F401
 from .criterion import HungarianMatcher, SetCriterion  # noqa: F401
 from .lxmert import LxmertEngine, GeneratorOurs, GeneratorBaselines, GeneratorOursAblationNoAggregation  # noqa: F401
 from .visualbert import VisualBertEngine, SelfAttentionGenerator  # noqa: F401
+from .visualize import show_image_relevance, generate_visualization, save_image_vis, show_heatmap_on_text  # noqa: F401
 from .perturbation import LxmertPerturbation, VisualBertPerturbation, PERT_STEPS, topk_select  # noqa: F401
 
 __all__ = ["MmxError", "lib", "interpret", "ClipEngine", "ClipConfig", "avg_heads", "avg_heads_batched",

@@ -137,6 +137,11 @@ _SIGS = {
     "mmx_detr_mask_losses": (C.c_int, [c_float_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p),
                                        C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int), C.c_void_p, c_float_p, c_float_p,
                                        C.c_void_p]),
+    "mmx_relevance_overlay": (C.c_int, [c_float_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, c_float_p, C.c_int,
+                                        C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "mmx_box_relevance_image": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, c_float_p, c_float_p, C.c_int, C.c_int,
+                                          C.c_void_p, C.c_void_p]),
+    "mmx_clip_text_scores": (C.c_int, [c_float_p, c_int_p, C.c_int, C.c_int, c_float_p, c_int_p, C.c_void_p]),
     "mmx_clip_create": (C.c_int, [C.POINTER(ClipConfigC), C.c_int, C.POINTER(C.c_void_p)]),
     "mmx_clip_destroy": (None, [C.c_void_p]),
     "mmx_clip_load_tensor": (C.c_int, [C.c_void_p, C.c_char_p, c_float_p, C.c_size_t]),
